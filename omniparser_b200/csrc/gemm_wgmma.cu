@@ -60,7 +60,7 @@ struct GemmArgs {
   int nb;                // images per tile (small maps: a TMA box spans nb consecutive images)
   int tw_valid;          // valid output columns per tile row (== tw except in halo mode, where tw is the halo pitch)
   int stagesA, cin;      // separate-pipeline modes: A ring depth; Cin
-  uint32_t a_slot;       // separate-pipeline modes: bytes per A slot
+  uint32_t a_slot;       // bytes per A slot (single ring: per A half, 128 rows x bk)
   // sep: A and B move through SEPARATE pipelines (always in halo mode 3, where one A tile feeds nine weight taps).
   // bres (implies sep): the WHOLE weight matrix of this launch (n_tiles == 1) stays resident in shared memory -- every B
   // k-block is loaded once per CTA, on its first work item, and the persistent loop afterwards streams only A tiles.  For
@@ -82,7 +82,9 @@ struct GemmArgs {
   int res_lo;  // > 0: the fp16 residual is a hi/lo pair too, lo at column res_lo + n
   // fp16x3 operands: A rows are [hi(K) | lo(K)] (conv: per pixel [hi(Cin) | lo(Cin)]), W rows [hi | lo] likewise.  Each
   // pipeline stage holds A_hi, A_lo, B_hi, B_lo of ONE logical k-block (each loaded once) and the consumers issue the
-  // three products hi*hi + hi*lo + lo*hi into the same fp32 accumulator.
+  // three products hi*hi + hi*lo + lo*hi into the same fp32 accumulator.  The k-blocks are 32 wide (64B swizzle): a
+  // 64-wide fp16x3 stage at BN=256 is 96 KiB, so only two would fit and one stage would load while the other is read;
+  // 32-wide stages give the ring four.  The k16 steps, and so every sum, run in the same order either way.
   int mt_fast;   // tile order: 1 = M tiles fastest (concurrent CTAs share a B tile: weights larger than activations, e.g. the LM head)
   int x3, lo_a, lo_b, b_tap;   // lo_a / lo_b: column offset of the lo half in A / B; b_tap: B columns per conv tap
   float* ws;   // split-K partial tiles [tile][slice][128][bn] fp32
@@ -294,7 +296,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t a_part = g.x3 ? 2u * kASlot : uint32_t(kASlot);                     // [A_hi][A_lo] | [A]
+  const uint32_t a_part = g.x3 ? 2u * g.a_slot : g.a_slot;                          // single ring: [A_hi][A_lo] | [A]
   const uint32_t stage_bytes = g.sep ? g.b_slot : a_part + (g.x3 ? 2u : 1u) * g.b_slot;
   const uint32_t a_region = g.sep ? uint32_t(g.stagesA) * g.a_slot : 0u;   // separate pipelines: [A slots][B slots]
   float* epi_stage = reinterpret_cast<float*>(smem + a_region + size_t(g.stages) * stage_bytes);   // [8 warps][16 rows][kStagePitch]
@@ -441,7 +443,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           bcol = tap * b_tap + c0;
         }
         for (int half = 0; half <= int(x3); ++half) {     // half 1 = the lo parts (fp16x3 operands only)
-          const uint32_t dst = sa + uint32_t(half) * kASlot;
+          const uint32_t dst = sa + uint32_t(half) * a_slot;
           const int ca = half * lo_a;
           if (mode == 0) {
             tma_load_2d_elect(dst, &tmA, fb, ca + kb * bk, mt * kTileM);
@@ -572,7 +574,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const uint32_t sb = sa + a_part;
         wgmma_fence_operand(acc);
         wgmma_fence();
-        if (x3) mma_stage_x3<BN>(acc, lo_of(sa) + wg_rows, lo_of(sa + kASlot) + wg_rows, lo_of(sb), lo_of(sb + b_slot), dhi, ksteps, row16, accum);
+        if (x3) mma_stage_x3<BN>(acc, lo_of(sa) + wg_rows, lo_of(sa + a_slot) + wg_rows, lo_of(sb), lo_of(sb + b_slot), dhi, ksteps, row16, accum);
         else if (bf16) mma_stage<BN, true>(acc, lo_of(sa) + wg_rows, lo_of(sb), dhi, ksteps, row16, accum);
         else mma_stage<BN, false>(acc, lo_of(sa) + wg_rows, lo_of(sb), dhi, ksteps, row16, accum);
         wgmma_commit();
@@ -952,7 +954,10 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   CUtensorMap tmA, tmB;
   const int Ktot = (d.mode == 0) ? d.K : 9 * d.Cin;
   const int kred = (d.mode == 0) ? d.K : d.Cin;
-  const int bk = (kred % 64 == 0) ? 64 : 32;
+  // fp16x3 operands always stream 32-wide k-blocks (GemmArgs::x3).  The tiling and split-K choice is still made for 64-wide
+  // blocks where K allows them (kb_merge = 2), so split-K slices start at the same K offsets and every sum keeps its order.
+  const int bk = (kred % 64 == 0 && !d.x3) ? 64 : 32;
+  const int kb_merge = (d.x3 && kred % 64 == 0) ? 2 : 1;
   if (d.mode != 0 && kred % 32 != 0) return set_error("conv3x3: Cin must be a multiple of 32");
   if (d.mode == 0 && (d.K % 8 != 0 || d.lda % 8 != 0)) return set_error("gemm: K and lda must be multiples of 8");
   if ((reinterpret_cast<uintptr_t>(d.A) & 15) || (reinterpret_cast<uintptr_t>(d.B) & 15)) return set_error("gemm: operands must be 16-byte aligned");
@@ -1060,7 +1065,8 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   int bn = 16, ksplit = 1;
   static const bool no_split = getenv("B2P_NO_SPLITK") != nullptr;
   const int slot = (no_split || d.no_split) ? -1 : ws_slot_for(st);
-  pick_tiling(d.N, g.m_tiles, g.num_kb, halo ? 9 * bk : bk, g.a_bytes, d.bn_max > 0 ? d.bn_max : 256, slot >= 0, d.x3 != 0, &bn, &ksplit);
+  pick_tiling(d.N, g.m_tiles, g.num_kb / kb_merge, (halo ? 9 * bk : bk) * kb_merge, g.a_bytes * kb_merge, d.bn_max > 0 ? d.bn_max : 256,
+              slot >= 0, d.x3 != 0, &bn, &ksplit);
   // Resident weights: one N tile, no split-K, at least one full wave of M tiles, and the whole weight matrix + a >= 2-deep
   // A ring must fit in shared memory (see GemmArgs::bres).
   static const bool no_res = getenv("B2P_NO_BRES") != nullptr;
@@ -1096,7 +1102,7 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   static const bool sk_last = getenv("B2P_SPLITK_LAST") != nullptr;
   g.sk_last = sk_last ? 1 : 0;
   g.ksplit = ksplit;
-  g.kb_per = (g.num_kb + ksplit - 1) / ksplit;
+  g.kb_per = kb_merge * ((g.num_kb / kb_merge + ksplit - 1) / ksplit);
   g.ws = slot >= 0 ? g_ws[slot] : nullptr;
   g.counters = slot >= 0 ? g_counters[slot] : nullptr;
   g.n_tiles = (d.N + bn - 1) / bn;
@@ -1114,7 +1120,8 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   g.d_ksplit = FastDiv::make(g.ksplit); g.d_ntiles = FastDiv::make(g.n_tiles); g.d_mtiles = FastDiv::make(g.m_tiles);
   g.d_perimg = FastDiv::make(d.mode != 0 ? g.tiles_x * g.tiles_y : 1); g.d_tilesx = FastDiv::make(d.mode != 0 ? g.tiles_x : 1);
   g.d_cinb = FastDiv::make(d.mode != 0 ? g.cin_blocks : 1);
-  const int stage_bytes = g.sep ? int(g.b_slot) : xk * (kASlot + int(g.b_slot));
+  if (!g.sep) g.a_slot = uint32_t(kTileM) * bk * 2;     // single ring: one A half per slot
+  const int stage_bytes = g.sep ? int(g.b_slot) : xk * (int(g.a_slot) + int(g.b_slot));
   int stages, bar_space = 512;
   if (bres) {
     g.a_slot = a_slot_sep;
