@@ -152,7 +152,10 @@ int b2p_decoder_embed(const float* E, const int* seq, int seq_ld, const int* ste
                       float* out, b2p_stream_t stream);
 int b2p_projector_prep(const float* x, const float* pos, int B, int HW, int C, void* out, int split,
                        b2p_stream_t stream);
-/* HF greedy step with no_repeat_ngram / forced BOS / forced EOS processors, hf:generation/utils.py:2727-2805 */
+/* HF greedy step with no_repeat_ngram / forced BOS / forced EOS processors, hf:generation/utils.py:2727-2805.  Writes
+ * seq[b][*step + 1]; *step + 1 must be <= max_len - 1.  The ban list is never truncated (up to max_len - 1 entries in
+ * shared memory).  Refused before any launch: B < 0, V < 1, ld < V, ngram < 0, max_len outside [2, 8192],
+ * seq_ld < max_len, forced ids >= V.  B == 0 launches nothing. */
 int b2p_greedy_pick(const float* logits, long long ld, int V, int B, int* seq, int seq_ld, int* finished,
                     const int* step, int ngram, int forced_bos, int forced_eos, int eos, int pad, int max_len,
                     float* dump, int* n_unfinished, b2p_stream_t stream);

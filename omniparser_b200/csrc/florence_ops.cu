@@ -638,7 +638,7 @@ __global__ void projector_prep_kernel(const float* __restrict__ x /*[B][HW][C]*/
 // HF greedy step (hf:generation/utils.py:2727-2805) with the processors Florence-2 configures, in HF order:
 // no_repeat_ngram (hf:generation/logits_process.py:1012-1079), forced BOS (:1552), forced EOS (:1597); then
 // argmax (first maximum), pad for finished rows, EOS bookkeeping.  seq[b][0] = decoder_start; this kernel writes
-// seq[b][*step + 1].  One CTA per row.
+// seq[b][*step + 1], *step + 1 <= max_len - 1.  One CTA per row.
 struct PickArgs {
   const float* logits; long long ld; int V;
   int* seq; int seq_ld;
@@ -649,6 +649,11 @@ struct PickArgs {
   int* n_unfinished;    // device counter, decremented when a row finishes
 };
 
+// The ban list lives in dynamic shared memory, max_len ints: a pick at length cur_len <= max_len - 1 bans at most
+// cur_len - ngram + 1 < max_len tokens (greedy decoding never repeats an n-gram, so a recurring (n-1)-gram prefix bans
+// one more distinct token every time it recurs: long generations do reach hundreds of bans).
+constexpr int kPickMaxLen = 8192;   // 32 KiB of bans
+
 __global__ void __launch_bounds__(1024) greedy_pick_kernel(PickArgs a) {
   pdl_wait();   // PDL: inputs come from the previous kernel in the stream
   const int b = blockIdx.x;
@@ -658,22 +663,25 @@ __global__ void __launch_bounds__(1024) greedy_pick_kernel(PickArgs a) {
   int* seq = a.seq + (long long)b * a.seq_ld;
   __shared__ float bv[32];
   __shared__ int bi[32];
-  __shared__ int banned[64];
-  __shared__ int nbanned;
-  if (threadIdx.x == 0) {
-    int nb = 0;
-    if (a.ngram > 0 && cur_len + 1 >= a.ngram) {
-      // ban every token that would complete an n-gram already present in seq[0..cur_len)
-      const int pre = a.ngram - 1;
-      for (int s = 0; s + a.ngram <= cur_len; ++s) {
-        bool eq = true;
-        for (int k = 0; k < pre; ++k) eq = eq && (seq[s + k] == seq[cur_len - pre + k]);
-        if (eq && nb < 64) banned[nb++] = seq[s + pre];
+  extern __shared__ int banned[];   // [max_len]
+  __shared__ int nbanned_s;
+  if (threadIdx.x == 0) nbanned_s = 0;
+  __syncthreads();
+  if (a.ngram > 0 && cur_len + 1 >= a.ngram) {
+    // ban every token that would complete an n-gram already present in seq[0..cur_len); one start position per thread
+    // (the list order does not matter: it is only tested for membership)
+    const int pre = a.ngram - 1;
+    for (int s = threadIdx.x; s + a.ngram <= cur_len; s += blockDim.x) {
+      bool eq = true;
+      for (int k = 0; k < pre; ++k) eq = eq && (seq[s + k] == seq[cur_len - pre + k]);
+      if (eq) {
+        const int i = atomicAdd(&nbanned_s, 1);
+        if (i < a.max_len) banned[i] = seq[s + pre];   // always true for cur_len <= max_len - 1
       }
     }
-    nbanned = nb;
   }
   __syncthreads();
+  const int nbanned = min(nbanned_s, a.max_len);
   int force = -1;
   if (cur_len == 1 && a.forced_bos >= 0) force = a.forced_bos;
   if (cur_len == a.max_len - 1 && a.forced_eos >= 0) force = a.forced_eos;
@@ -682,7 +690,7 @@ __global__ void __launch_bounds__(1024) greedy_pick_kernel(PickArgs a) {
   if (a.dump || force < 0) {
     const bool vec = !a.dump && force < 0 && (a.ld % 2 == 0) && ((reinterpret_cast<uintptr_t>(lg) & 7) == 0);
     if (vec) {
-      // plain scan; the (<= 19-entry) ban list is only consulted when a value would become the running maximum
+      // plain scan; the ban list is only consulted when a value would become the running maximum
       const float2* lp = reinterpret_cast<const float2*>(lg);
       const int V2 = a.V >> 1;
       // four strided loads in flight per thread before the compares (one load per iteration left every thread waiting on an
@@ -934,11 +942,18 @@ int b2p_projector_prep(const float* x, const float* pos, int B, int HW, int C, v
 int b2p_greedy_pick(const float* logits, long long ld, int V, int B, int* seq, int seq_ld, int* finished,
                     const int* step, int ngram, int forced_bos, int forced_eos, int eos, int pad, int max_len,
                     float* dump, int* n_unfinished, cudaStream_t st) {
+  if (B < 0) return set_error("greedy_pick: B must be >= 0");
+  if (B == 0) return 0;
+  if (V < 1 || ld < V) return set_error("greedy_pick: need 1 <= V <= ld");
+  if (ngram < 0) return set_error("greedy_pick: ngram must be >= 0 (0 = no n-gram ban)");
+  if (max_len < 2 || max_len > kPickMaxLen) return set_error("greedy_pick: max_len must be in [2, 8192]");
+  if (seq_ld < max_len) return set_error("greedy_pick: seq_ld must be >= max_len");
+  if (forced_bos >= V || forced_eos >= V) return set_error("greedy_pick: forced token ids must be < V");
   PickArgs a{};
   a.logits = logits; a.ld = ld; a.V = V; a.seq = seq; a.seq_ld = seq_ld; a.finished = finished; a.step = step;
   a.ngram = ngram; a.forced_bos = forced_bos; a.forced_eos = forced_eos; a.eos = eos; a.pad = pad; a.max_len = max_len;
   a.dump = dump; a.n_unfinished = n_unfinished;
-  launch_pdl(greedy_pick_kernel, dim3(B), dim3(1024), 0, st, a);
+  launch_pdl(greedy_pick_kernel, dim3(B), dim3(1024), size_t(max_len) * sizeof(int), st, a);
   B2P_CHECK_LAUNCH();
   return 0;
 }

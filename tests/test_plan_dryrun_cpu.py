@@ -89,6 +89,10 @@ def _check(name, a):
     elif name == "b2p_layernorm":
         _x, ldx, _g, _b, eps, T, Cc, o16, ld16, o32, ld32, split, _st = a
         assert ldx >= Cc and (o16 is None or ld16 >= (2 if split else 1) * Cc) and (o32 is None or ld32 >= Cc)
+    elif name == "b2p_greedy_pick":
+        _lg, ld, V, B, _seq, seq_ld, _fin, _step, ngram, bos, feos, _eos, _pad, max_len, _dump, _nunf, _st = a
+        assert B >= 0 and 1 <= V <= ld and ngram >= 0 and 2 <= max_len <= 8192 and seq_ld >= max_len, (V, ld, ngram, max_len, seq_ld)
+        assert bos < V and feos < V
     elif name in ("b2p_dwconv_ln", "b2p_channel_attn", "b2p_window_attn", "b2p_mha", "b2p_mha_cached", "b2p_projector_prep"):
         split = a[-2]
         assert 0 <= split <= 7            # bit 0: [hi | lo] output, bit 1: round-2 tile/small variants, bit 2: florence_simt.cu kernels
