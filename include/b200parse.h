@@ -161,6 +161,57 @@ int b2p_greedy_pick(const float* logits, long long ld, int V, int B, int* seq, i
                     float* dump, int* n_unfinished, b2p_stream_t stream);
 int b2p_step_advance(int* step, b2p_stream_t stream);
 
+/* ---- Florence-2 beam search, HF's _beam_search (hf:generation/utils.py:3076-3386, helpers :2876-3072) ----
+ * Decoder rows r = crop * nb + beam (B = K * nb), 1 <= nb <= 16; decoder prompt length 1 (decoder_start at seq[r][0]).
+ *
+ * Tie rule (ours: torch.topk leaves the order of exact ties unspecified): every selection takes the higher score first and,
+ * on equal scores, the lower index -- the flat index beam * V + token in the per-crop top 2 nb, the position in that list when
+ * the running beams are picked, the merged index (old hypotheses 0..nb-1, then candidates) when hypotheses are merged.
+ * Two kinds of ties that torch may break differently never reach the output:
+ *  - the -1e9 placeholders (initial beams 1..nb-1, and candidates that did not finish, whose s / L^lp - 1e9 rounds to
+ *    -1e9 in fp32): a crop stops only when every hypothesis slot holds a finished sequence with a real score (the early-stop
+ *    heuristic cannot fail while a slot is empty, and at max_len the top nb candidates all finish), and tied placeholder
+ *    running beams share the same prefix and cache contents;
+ *  - the -inf candidates of a forced step (forced BOS / EOS leave one finite score per beam): they only fill ranks >= nb,
+ *    which neither become running beams nor finish.
+ *
+ * b2p_beam_topk (HF step b + the per-row part of c): per row, log_softmax of logits[r][0..V) in fp32, then the processors on
+ * the log-probs in HF order -- no_repeat_ngram bans -> -inf (the ban scan is greedy_pick's), forced BOS / EOS: -inf except the
+ * forced token's 0 (the logits are then not read) -- plus bscore[r]; writes the row's best 2 nb as cand_score / cand_idx
+ * [B][2 nb] (flat index beam * V + token), best first.  The crop's top 2 nb lies in the union of its rows' top 2 nb.  Rows of
+ * crops with done[crop] set are skipped (done may be null).  Refused before any launch: B < 0, nb outside [1, 16],
+ * B % nb != 0, V < 2 nb, ld < V, ngram < 0, max_len outside [2, 8192], seq_ld < max_len, forced ids >= V.  B == 0 launches
+ * nothing. */
+int b2p_beam_topk(const float* logits, long long ld, int V, int B, int nb, const int* seq, int seq_ld, const int* step,
+                  int ngram, int forced_bos, int forced_eos, int max_len, const float* bscore, const int* done,
+                  float* cand_score, int* cand_idx, b2p_stream_t stream);
+/* b2p_beam_update (HF steps c-g; one CTA per crop, crops with done[k] set are left untouched -- their hypotheses can no
+ * longer change): merges the rows' candidates to the crop's top 2 nb; flags EOS / max-length hits; picks the running beams
+ * (score + hit * -1e9, best nb: _get_running_beams_for_next_iteration :2995-3016); merges finished hypotheses
+ * (_update_finished_beams :3018-3072: / L^lp, the "batch full" and heuristic -1e9 terms, top-nb mask, in fp32 and in HF's
+ * order); updates the early-stop heuristic (_check_early_stop_heuristic :2876-2925; early_stopping 0 = False, 1 = True,
+ * 2 = "never", only the sign of length_penalty is used); then writes the new tokens and parent-gathered prefixes into seq,
+ * bscore, parent[r] (beam index, may be null) and the cache ancestor table src[r][0..t] (src'[r][j] = src[parent][j] for j < t,
+ * src'[r][t] = the parent's row), and, when the crop stops (_beam_search_has_unfinished_sequences :2927-2949 for the crop),
+ * sets done[k] and decrements *n_open.  lp_pow[L] = float(L ** length_penalty) computed in double (torch divides fp32 by the
+ * Python float).  Finished hypotheses: hyp_seq [K * nb][seq_ld] (pad-filled), hyp_score / hyp_len (generated tokens incl.
+ * EOS) / hyp_fin [K * nb], best first.  Initial state: bscore [0, -1e9, ...] per crop, hyp_score -1e9, hyp_fin 0, hyp_seq pad,
+ * heur 1.  The crop's seq and src rows are staged in shared memory, so nb * max_len is limited to 16384.  Refused before any
+ * launch: K < 0, nb outside [1, 16], V < 2 nb, max_len outside [2, 8192], seq_ld < max_len, tmax < max_len - 1,
+ * nb * max_len > 16384, early_stopping outside {0, 1, 2}, lp_pow null.  K == 0 launches nothing. */
+int b2p_beam_update(const float* cand_score, const int* cand_idx, int V, int K, int nb, int* seq, int seq_ld, int* src,
+                    int tmax, const int* step, int eos, int pad, int max_len, int early_stopping, float length_penalty,
+                    const float* lp_pow, float* bscore, int* parent, int* hyp_seq, float* hyp_score, int* hyp_len,
+                    int* hyp_fin, int* heur, int* done, int* n_open, b2p_stream_t stream);
+/* b2p_mha_cached with a beam-indexed cache instead of HF's reorder_cache (hf:generation/utils.py:3340-3346): row r's entry for
+ * position j < *step is read from physical row src[r][j] ([B][tmax]); this step's k / v are appended at (r, *step). */
+int b2p_mha_cached_beam(const float* q, long long ldq, const float* knew, const float* vnew, long long ldnew, float* kcache,
+                        float* vcache, int tmax, const int* step, const int* src, int B, int heads, void* out, long long ldo,
+                        int split, b2p_stream_t stream);
+/* b2p_mha where query row b reads K / V batch b / rows_per_kv (the crop's cross-attention K / V, shared by its beams). */
+int b2p_mha_grouped(const float* q, long long ldq, const float* k, const float* v, long long ldk, int B, int Lq, int Lk,
+                    int heads, int rows_per_kv, void* out, long long ldo, int split, b2p_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

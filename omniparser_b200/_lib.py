@@ -59,6 +59,11 @@ PROTOTYPES = {
     "b2p_projector_prep": (i32, [vp, vp, i32, i32, i32, vp, i32, vp]),
     "b2p_greedy_pick": (i32, [vp, i64, i32, i32, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
     "b2p_step_advance": (i32, [vp, vp]),
+    "b2p_beam_topk": (i32, [vp, i64, i32, i32, i32, vp, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp]),
+    "b2p_beam_update": (i32, [vp, vp, i32, i32, i32, vp, i32, vp, i32, vp, i32, i32, i32, i32, f32, vp, vp, vp, vp, vp, vp,
+                              vp, vp, vp, vp, vp]),
+    "b2p_mha_cached_beam": (i32, [vp, i64, vp, vp, i64, vp, vp, i32, vp, vp, i32, i32, vp, i64, i32, vp]),
+    "b2p_mha_grouped": (i32, [vp, i64, vp, vp, i64, i32, i32, i32, i32, i32, vp, i64, i32, vp]),
 }
 
 

@@ -32,6 +32,27 @@ DEFAULT_GEN = dict(forced_bos_token_id=0, forced_eos_token_id=2, no_repeat_ngram
                    bos_token_id=0, decoder_start_token_id=2)
 BUCKET = 32
 BUCKET_768 = 16      # 768x768 mode: 36864 stage-0 tokens per crop -> small chunks (activations ~1.5 GB per crop)
+BEAM_DEFAULTS = dict(early_stopping=False, length_penalty=1.0)   # transformers GenerationConfig defaults
+
+
+def beam_settings(num_beams=1, do_sample=False, early_stopping=None, length_penalty=None, num_return_sequences=1,
+                  defaults: Optional[dict] = None) -> dict:
+    """Validated decoding settings of ``generate``: greedy (num_beams == 1) or HF beam search with 2..16 beams.  Omitted
+    early_stopping / length_penalty come from ``defaults`` (the checkpoint's generation config)."""
+    if do_sample:
+        raise NotImplementedError("sampling (do_sample=True) is not on the hot path: greedy or beam search only")
+    if not isinstance(num_beams, int) or not 1 <= num_beams <= 16:
+        raise ValueError(f"num_beams must be an int in [1, 16], got {num_beams!r}")
+    if not isinstance(num_return_sequences, int) or not 1 <= num_return_sequences <= num_beams:
+        raise ValueError(f"num_return_sequences must be in [1, num_beams = {num_beams}], got {num_return_sequences!r}")
+    d = dict(BEAM_DEFAULTS, **(defaults or {}))
+    es = d["early_stopping"] if early_stopping is None else early_stopping
+    lp = d["length_penalty"] if length_penalty is None else length_penalty
+    if not (es is True or es is False or es == "never"):   # HF tests `early_stopping is True`: 0 / 1 are not booleans here
+        raise ValueError(f"early_stopping must be True, False or 'never', got {es!r}")
+    if num_beams == 1:   # greedy: the beam settings do not apply and stay out of the plan key
+        return dict(num_beams=1, num_return_sequences=1)
+    return dict(num_beams=num_beams, early_stopping=es, length_penalty=float(lp), num_return_sequences=num_return_sequences)
 
 
 class _Batch(dict):
@@ -84,8 +105,14 @@ class B200Florence2Processor:
 
 
 class B200Florence2Model:
+    beam_defaults = BEAM_DEFAULTS
+
     def __init__(self, state_dict: Dict[str, torch.Tensor], device, gen_cfg: Optional[dict] = None,
-                 precision: str = "fp16x3", name_or_path: str = "b200/florence2", use_graph: bool = True):
+                 precision: str = "fp16x3", name_or_path: str = "b200/florence2", use_graph: bool = True,
+                 beam_defaults: Optional[dict] = None):
+        """beam_defaults: ``early_stopping`` / ``length_penalty`` that ``generate(num_beams > 1)`` uses when the call omits
+        them (:func:`load_beam_defaults` reads them from a checkpoint's generation config; HF's own defaults otherwise)."""
+        self.beam_defaults = dict(BEAM_DEFAULTS, **(beam_defaults or {}))
         self.device = torch.device(device)
         if self.device.type != "cuda" or not torch.cuda.is_available():
             raise RuntimeError("Florence-2 needs a CUDA device; there is no CPU fallback")
@@ -112,30 +139,43 @@ class B200Florence2Model:
     def eval(self):
         return self
 
-    def plan_for(self, n: int, max_new_tokens: int, prompt_ids: Sequence[int], size: int = 64, instance: int = 0) -> FlorencePlan:
-        """Launch plan (buffers + CUDA graphs) for up to ``n`` crops.  Plans of different ``instance`` share nothing
-        mutable, so the pipeline can caption two batches concurrently on two streams."""
+    def _plan_key(self, n, max_new_tokens, prompt_ids, size, instance, num_beams, early_stopping, length_penalty):
+        """(plan key, validated beam settings); omitted early_stopping / length_penalty resolve through ``beam_defaults``
+        exactly as in ``generate``, so a plan warmed without them is the one ``generate`` uses"""
         if size == 64:
             K = max(BUCKET, ((n + BUCKET - 1) // BUCKET) * BUCKET)
         else:
             K = BUCKET_768
-        key = (K, max_new_tokens, tuple(prompt_ids), size, instance)
+        bs = beam_settings(num_beams, False, early_stopping, length_penalty, 1, self.beam_defaults)
+        del bs["num_return_sequences"]
+        beam = (num_beams, bs["early_stopping"], bs["length_penalty"]) if num_beams > 1 else ()
+        return (K, max_new_tokens, tuple(prompt_ids), size, instance) + beam, bs
+
+    def plan_for(self, n: int, max_new_tokens: int, prompt_ids: Sequence[int], size: int = 64, instance: int = 0, *,
+                 num_beams: int = 1, early_stopping=None, length_penalty=None) -> FlorencePlan:
+        """Launch plan (buffers + CUDA graphs) for up to ``n`` crops.  Plans of different ``instance`` share nothing
+        mutable, so the pipeline can caption two batches concurrently on two streams.  num_beams > 1: a beam-search plan
+        (early_stopping / length_penalty are part of it, defaulting to ``beam_defaults``; greedy plans ignore them)."""
+        key, bs = self._plan_key(n, max_new_tokens, prompt_ids, size, instance, num_beams, early_stopping, length_penalty)
         with self._plan_lock:
             if key not in self._plans:
                 with torch.cuda.device(self.device):
-                    self._plans[key] = FlorencePlan(self.weights, K, max_new_tokens, list(prompt_ids), self.use_graph, size, instance)
+                    self._plans[key] = FlorencePlan(self.weights, key[0], max_new_tokens, list(prompt_ids), self.use_graph, size, instance,
+                                                    **bs)
             return self._plans[key]
 
-    def plan_ready(self, n: int, max_new_tokens: int, prompt_ids: Sequence[int], size: int = 64, instance: int = 0) -> bool:
-        K = max(BUCKET, ((n + BUCKET - 1) // BUCKET) * BUCKET) if size == 64 else BUCKET_768
-        p = self._plans.get((K, max_new_tokens, tuple(prompt_ids), size, instance))
+    def plan_ready(self, n: int, max_new_tokens: int, prompt_ids: Sequence[int], size: int = 64, instance: int = 0, *,
+                   num_beams: int = 1, early_stopping=None, length_penalty=None) -> bool:
+        p = self._plans.get(self._plan_key(n, max_new_tokens, prompt_ids, size, instance, num_beams, early_stopping, length_penalty)[0])
         return p is not None and (p.warmed or not p.use_graph)
 
     @torch.inference_mode()
-    def warm_plan(self, n: int, max_new_tokens: int, prompt_ids: Sequence[int], size: int = 64, instance: int = 0, stream=None):
+    def warm_plan(self, n: int, max_new_tokens: int, prompt_ids: Sequence[int], size: int = 64, instance: int = 0, stream=None, *,
+                  num_beams: int = 1, early_stopping=None, length_penalty=None):
         """Construct the plan for this crop-count bucket and capture its graphs on scratch inputs."""
         with torch.cuda.device(self.device), torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream()):
-            self.plan_for(n, max_new_tokens, prompt_ids, size, instance).warm()
+            self.plan_for(n, max_new_tokens, prompt_ids, size, instance, num_beams=num_beams, early_stopping=early_stopping,
+                          length_penalty=length_penalty).warm()
 
     def _to_u8(self, pixel_values: torch.Tensor) -> torch.Tensor:
         if pixel_values.dtype == torch.uint8:
@@ -148,9 +188,11 @@ class B200Florence2Model:
         return ((x * std + mean) * 255.0).round().clamp(0, 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
 
     @torch.inference_mode()
-    def generate_from_device_crops(self, plan: FlorencePlan, n: int, sync_every: int = 4, from_resized: bool = False) -> torch.Tensor:
+    def generate_from_device_crops(self, plan: FlorencePlan, n: int, sync_every: int = 4, from_resized: bool = False,
+                                   num_return_sequences: int = 1) -> torch.Tensor:
         """Crops already in ``plan.crops[:n]`` (device; ``plan.crops_in`` if from_resized).  Returns LongTensor [n, T] on
-        the device, HF layout ``[decoder_start, tokens..., eos, pad...]`` truncated where every row has finished."""
+        the device, HF layout ``[decoder_start, tokens..., eos, pad...]`` truncated where every row has finished.  A beam
+        plan returns [n * num_return_sequences, 1 + longest returned hypothesis], best first within each crop."""
         with plan.lock, torch.cuda.device(self.device):   # a plan instance (buffers + graphs) serves one generation at a time
             if n < plan.K:
                 (plan.crops_in if from_resized else plan.crops)[n:].zero_()
@@ -163,6 +205,8 @@ class B200Florence2Model:
                 if steps % sync_every == 0 and steps < plan.T and plan.unfinished() == 0:
                     break
             plan.join()
+            if plan.nb > 1:   # every crop is done by the last step (max-length hits), or was when the loop stopped
+                return plan.beam_sequences(n, num_return_sequences)
             # exact stop length: first step after which no row was unfinished
             seq = plan.seq[:n, :steps + 1]
             if steps > 1:
@@ -182,14 +226,17 @@ class B200Florence2Model:
         return last if last < seq.shape[1] else None
 
     @torch.inference_mode()
-    def generate(self, input_ids=None, pixel_values=None, max_new_tokens=20, num_beams=1, do_sample=False, **kw):
-        """ref:util/utils.py:125."""
-        if num_beams != 1 or do_sample:
-            raise NotImplementedError("only greedy decoding (num_beams=1, do_sample=False) is on the hot path")
+    def generate(self, input_ids=None, pixel_values=None, max_new_tokens=20, num_beams=1, do_sample=False, early_stopping=None,
+                 length_penalty=None, num_return_sequences=1, **kw):
+        """ref:util/utils.py:125.  num_beams 2..16: HF beam search (hf:generation/utils.py:3076-3386) with the checkpoint's
+        processors; early_stopping / length_penalty default to ``beam_defaults``.  Returns HF's layout."""
+        bs = beam_settings(num_beams, do_sample, early_stopping, length_penalty, num_return_sequences, self.beam_defaults)
         with self._lock:
-            return self._generate(input_ids, pixel_values, max_new_tokens)
+            return self._generate(input_ids, pixel_values, max_new_tokens, bs)
 
-    def _generate(self, input_ids, pixel_values, max_new_tokens):
+    def _generate(self, input_ids, pixel_values, max_new_tokens, bs=None):
+        bs = dict(bs or dict(num_beams=1, num_return_sequences=1))
+        nrs = bs.pop("num_return_sequences")
         u8 = self._to_u8(pixel_values)
         n = u8.shape[0]
         if n == 0:
@@ -199,28 +246,46 @@ class B200Florence2Model:
             raise NotImplementedError("all rows must share one prompt (the reference passes [prompt]*len(batch))")
         side = int(u8.shape[1])
         if side == 64:
-            plan = self.plan_for(n, max_new_tokens, prompt)
+            plan = self.plan_for(n, max_new_tokens, prompt, **bs)
             plan.crops[:n].copy_(u8.to(self.device, non_blocking=True))
-            return self.generate_from_device_crops(plan, n)
+            return self.generate_from_device_crops(plan, n, num_return_sequences=nrs)
         if side != 768:
             raise ValueError("pixel_values must be 64x64 (do_resize=False) or 768x768 (processor default)")
-        return self.generate_chunked(u8, max_new_tokens, prompt, from_resized=True)
+        return self.generate_chunked(u8, max_new_tokens, prompt, from_resized=True, num_return_sequences=nrs, **bs)
 
     @torch.inference_mode()
-    def generate_chunked(self, crops_u8: torch.Tensor, max_new_tokens: int, prompt, from_resized: bool) -> torch.Tensor:
+    def generate_chunked(self, crops_u8: torch.Tensor, max_new_tokens: int, prompt, from_resized: bool, *, num_beams: int = 1,
+                         early_stopping=None, length_penalty=None, num_return_sequences: int = 1) -> torch.Tensor:
         """768x768 mode: run the crops through the (small-K) plan chunk by chunk; HF pads the shorter chunks with pad."""
         n = crops_u8.shape[0]
-        plan = self.plan_for(n, max_new_tokens, prompt, 768)
+        plan = self.plan_for(n, max_new_tokens, prompt, 768, num_beams=num_beams, early_stopping=early_stopping,
+                             length_penalty=length_penalty)
         outs = []
         for c0 in range(0, n, plan.K):
             m = min(plan.K, n - c0)
             dst = plan.crops_in if from_resized else plan.crops
             dst[:m].copy_(crops_u8[c0:c0 + m].to(self.device, non_blocking=True))
-            outs.append(self.generate_from_device_crops(plan, m, from_resized=from_resized).clone())
+            outs.append(self.generate_from_device_crops(plan, m, from_resized=from_resized,
+                                                        num_return_sequences=num_return_sequences).clone())
         width = max(o.shape[1] for o in outs)
         pad = self.gen["pad_token_id"]
         outs = [torch.nn.functional.pad(o, (0, width - o.shape[1]), value=pad) for o in outs]
         return torch.cat(outs, 0)
+
+
+def load_beam_defaults(path: str | Path) -> dict:
+    """``early_stopping`` / ``length_penalty`` of a local checkpoint directory's ``generation_config.json`` (then
+    ``config.json``), for ``B200Florence2Model(beam_defaults=)``; keys the files do not set are left out."""
+    out = {}
+    for name in ("generation_config.json", "config.json"):
+        f = Path(path) / name
+        if f.is_file():
+            cfg = json.loads(f.read_text())
+            for src in (cfg, cfg.get("text_config") or {}):
+                for k in BEAM_DEFAULTS:
+                    if k in src and src[k] is not None and k not in out:
+                        out[k] = src[k]
+    return out
 
 
 def load_florence_state(path: str | Path):

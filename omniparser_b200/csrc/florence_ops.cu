@@ -500,8 +500,14 @@ struct MhaArgs {
   const int* step;
   int B, Lq, Lk, heads;
   __half* out; long long ldo; int split;
+  const int* src; int rows_per_kv;                    // beam layout only (kBeam), see below
 };
 
+// kBeam = false: the greedy decoder / encoder layout above.  kBeam = true, beam search (R = crops * num_beams rows):
+//  - cached: row b's cache entry for position j < *step lives in physical row src[b][j] (src [B][tmax], kept by
+//    b2p_beam_update), the current position in row b itself, so a beam reorder never moves the caches;
+//  - explicit K / V: row b reads batch b / rows_per_kv (the cross-attention K / V of its crop, shared by its beams).
+template <bool kBeam>
 __global__ void mha_kernel(MhaArgs a) {
   pdl_wait();   // PDL: inputs come from the previous kernel in the stream
   const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -517,8 +523,10 @@ __global__ void mha_kernel(MhaArgs a) {
   int Lk = a.Lk;
   const float *kb, *vb;
   long long ldk;
+  const int* srow = nullptr;   // kBeam, cached: physical cache row of every position < t
+  int t = 0;
   if (a.kcache) {
-    const int t = *a.step;
+    t = *a.step;
     // append this step's k, v
     const float2 kn = *reinterpret_cast<const float2*>(a.knew + (long long)b * a.ldnew + h * 64 + 2 * lane);
     const float2 vn = *reinterpret_cast<const float2*>(a.vnew + (long long)b * a.ldnew + h * 64 + 2 * lane);
@@ -529,11 +537,22 @@ __global__ void mha_kernel(MhaArgs a) {
     kb = a.kcache + (long long)b * a.tmax * HD + h * 64;
     vb = a.vcache + (long long)b * a.tmax * HD + h * 64;
     ldk = HD;
+    if (kBeam) {
+      srow = a.src + (long long)b * a.tmax;
+      kb = a.kcache + h * 64;
+      vb = a.vcache + h * 64;
+    }
   } else {
-    kb = a.k + (long long)b * a.Lk * a.ldk + h * 64;
-    vb = a.v + (long long)b * a.Lk * a.ldk + h * 64;
+    const int bk = kBeam ? b / a.rows_per_kv : b;
+    kb = a.k + (long long)bk * a.Lk * a.ldk + h * 64;
+    vb = a.v + (long long)bk * a.Lk * a.ldk + h * 64;
     ldk = a.ldk;
   }
+  // offset of key / value row j from kb / vb
+  auto koff = [&](int jj) -> long long {
+    if (kBeam && srow) return ((long long)(jj < t ? srow[jj] : b) * a.tmax + jj) * HD;
+    return (long long)jj * ldk;
+  };
   float m = -INFINITY, l = 0.f;
   float2 acc = make_float2(0.f, 0.f);
   int j = 0;
@@ -544,8 +563,9 @@ __global__ void mha_kernel(MhaArgs a) {
     float s[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      kf[u] = *reinterpret_cast<const float2*>(kb + (long long)(j + u) * ldk + 2 * lane);
-      vf[u] = *reinterpret_cast<const float2*>(vb + (long long)(j + u) * ldk + 2 * lane);
+      const long long o = koff(j + u);
+      kf[u] = *reinterpret_cast<const float2*>(kb + o + 2 * lane);
+      vf[u] = *reinterpret_cast<const float2*>(vb + o + 2 * lane);
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) s[u] = q.x * kf[u].x + q.y * kf[u].y;
@@ -567,11 +587,12 @@ __global__ void mha_kernel(MhaArgs a) {
     m = mn;
   }
   for (; j < Lk; ++j) {
-    const float2 kf = *reinterpret_cast<const float2*>(kb + j * ldk + 2 * lane);
+    const long long o = koff(j);
+    const float2 kf = *reinterpret_cast<const float2*>(kb + o + 2 * lane);
     const float s = warp_sum(q.x * kf.x + q.y * kf.y);
     const float mn = fmaxf(m, s);
     const float r = __expf(m - mn), p = __expf(s - mn);
-    const float2 vf = *reinterpret_cast<const float2*>(vb + j * ldk + 2 * lane);
+    const float2 vf = *reinterpret_cast<const float2*>(vb + o + 2 * lane);
     l = l * r + p;
     acc.x = acc.x * r + p * vf.x;
     acc.y = acc.y * r + p * vf.y;
@@ -654,6 +675,24 @@ struct PickArgs {
 // one more distinct token every time it recurs: long generations do reach hundreds of bans).
 constexpr int kPickMaxLen = 8192;   // 32 KiB of bans
 
+// No-repeat-n-gram ban scan (hf:generation/logits_process.py:1012-1079) of one row, shared by the greedy pick and the beam
+// top-k: appends to banned[] every token that would complete an n-gram already present in seq[0..cur_len), one start
+// position per thread (the list order does not matter: it is only tested for membership).  *nbanned_s must be 0 and
+// visible to the whole CTA on entry; the caller synchronises before reading the list.
+__device__ __forceinline__ void ngram_bans(const int* seq, int cur_len, int ngram, int max_len, int* banned, int* nbanned_s) {
+  if (ngram > 0 && cur_len + 1 >= ngram) {
+    const int pre = ngram - 1;
+    for (int s = threadIdx.x; s + ngram <= cur_len; s += blockDim.x) {
+      bool eq = true;
+      for (int k = 0; k < pre; ++k) eq = eq && (seq[s + k] == seq[cur_len - pre + k]);
+      if (eq) {
+        const int i = atomicAdd(nbanned_s, 1);
+        if (i < max_len) banned[i] = seq[s + pre];   // always true for cur_len <= max_len - 1
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(1024) greedy_pick_kernel(PickArgs a) {
   pdl_wait();   // PDL: inputs come from the previous kernel in the stream
   const int b = blockIdx.x;
@@ -667,19 +706,7 @@ __global__ void __launch_bounds__(1024) greedy_pick_kernel(PickArgs a) {
   __shared__ int nbanned_s;
   if (threadIdx.x == 0) nbanned_s = 0;
   __syncthreads();
-  if (a.ngram > 0 && cur_len + 1 >= a.ngram) {
-    // ban every token that would complete an n-gram already present in seq[0..cur_len); one start position per thread
-    // (the list order does not matter: it is only tested for membership)
-    const int pre = a.ngram - 1;
-    for (int s = threadIdx.x; s + a.ngram <= cur_len; s += blockDim.x) {
-      bool eq = true;
-      for (int k = 0; k < pre; ++k) eq = eq && (seq[s + k] == seq[cur_len - pre + k]);
-      if (eq) {
-        const int i = atomicAdd(&nbanned_s, 1);
-        if (i < a.max_len) banned[i] = seq[s + pre];   // always true for cur_len <= max_len - 1
-      }
-    }
-  }
+  ngram_bans(seq, cur_len, a.ngram, a.max_len, banned, &nbanned_s);
   __syncthreads();
   const int nbanned = min(nbanned_s, a.max_len);
   int force = -1;
@@ -760,6 +787,289 @@ __global__ void __launch_bounds__(1024) greedy_pick_kernel(PickArgs a) {
 __global__ void step_advance_kernel(int* step) {
   pdl_wait();
   *step += 1;
+}
+
+// ---------------------------------------------------------------------------------------- beam search
+// HF beam search (hf:generation/utils.py:3076-3386, helpers :2876-3072) for decoder rows r = crop * nb + beam.  Tie rule
+// of every selection: higher score first, on equal scores the lower index (flat index beam * V + token in the top-k, position
+// in the list for the later selections).  See include/b200parse.h for why the ties torch.topk may order differently never
+// reach the output.
+constexpr int kBeamMax = 16;
+constexpr int kBeamSeqInts = 16384;   // staged seq + src rows of one crop: nb * max_len ints each (64 KiB)
+
+__device__ __forceinline__ bool beam_before(float v, int i, float w, int j) { return v > w || (v == w && i < j); }
+
+struct BeamTopkArgs {
+  const float* logits; long long ld; int V; int nb;
+  const int* seq; int seq_ld; const int* step;
+  int ngram, forced_bos, forced_eos, max_len;
+  const float* bscore;      // [B] running beam scores
+  const int* done;          // [B / nb] crops whose hypotheses are final (skipped); may be null
+  float* cand_score;        // [B][2 nb] best continuations of the row, best first
+  int* cand_idx;            // [B][2 nb] flat index beam * V + token
+};
+
+// One CTA per row: log_softmax in fp32, the processors on the log-probs (n-gram bans -> -inf; a forced step is -inf except the
+// forced token's 0, without reading the logits), + the row's running score, best 2 nb.  Each thread keeps its best M in
+// registers (M >= 2 nb, a power of two); the CTA then pops the best head 2 nb times.
+template <int M>
+__global__ void __launch_bounds__(256) beam_topk_kernel(BeamTopkArgs a) {
+  pdl_wait();
+  const int r = blockIdx.x, beam = r % a.nb, need = 2 * a.nb;
+  if (a.done && a.done[r / a.nb]) return;
+  const int t = *a.step, cur_len = t + 1;
+  const float* lg = a.logits + (long long)r * a.ld;
+  const int* seq = a.seq + (long long)r * a.seq_ld;
+  const float bs = a.bscore[r];
+  const int fbase = beam * a.V;
+  float* co = a.cand_score + (long long)r * need;
+  int* ci = a.cand_idx + (long long)r * need;
+  int force = -1;
+  if (cur_len == 1 && a.forced_bos >= 0) force = a.forced_bos;
+  if (cur_len == a.max_len - 1 && a.forced_eos >= 0) force = a.forced_eos;
+  if (force >= 0) {
+    // forced token first (0 + beam score), then -inf for the lowest other token ids (hf:generation/logits_process.py:1552,1597)
+    for (int j = threadIdx.x; j < need; j += blockDim.x) {
+      const int tok = j == 0 ? force : j - 1 + (j - 1 >= force ? 1 : 0);
+      co[j] = j == 0 ? 0.f + bs : -INFINITY;
+      ci[j] = fbase + tok;
+    }
+    return;
+  }
+  extern __shared__ int banned[];   // [max_len]
+  __shared__ int nbanned_s;
+  __shared__ float red_m[8], red_s[8];
+  __shared__ float win_v[2][8];
+  __shared__ int win_i[2][8];
+  if (threadIdx.x == 0) nbanned_s = 0;
+  __syncthreads();
+  ngram_bans(seq, cur_len, a.ngram, a.max_len, banned, &nbanned_s);
+  // log-sum-exp of the raw logits (online max / sum per thread, then across the CTA)
+  float m = -INFINITY, s = 0.f;
+  for (int v = threadIdx.x; v < a.V; v += blockDim.x) {
+    const float x = lg[v];
+    if (x > m) { s = s * expf(m - x) + 1.f; m = x; }
+    else if (x > -INFINITY) s += expf(x - m);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  for (int o = 16; o; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o), os = __shfl_xor_sync(0xffffffffu, s, o);
+    const float mn = fmaxf(m, om);
+    s = (m > -INFINITY ? s * expf(m - mn) : 0.f) + (om > -INFINITY ? os * expf(om - mn) : 0.f);
+    m = mn;
+  }
+  if (lane == 0) { red_m[warp] = m; red_s[warp] = s; }
+  __syncthreads();   // also publishes the ban list
+  float mx = -INFINITY;
+  for (int w = 0; w < nwarp; ++w) mx = fmaxf(mx, red_m[w]);
+  float sum = 0.f;
+  for (int w = 0; w < nwarp; ++w) if (red_m[w] > -INFINITY) sum += red_s[w] * expf(red_m[w] - mx);
+  const float lse = logf(sum);
+  const int nbanned = min(nbanned_s, a.max_len);
+  // per-thread best M of (log_softmax + bans) + beam score, ascending token order within the thread
+  float tv[M];
+  int ti[M];
+#pragma unroll
+  for (int k = 0; k < M; ++k) { tv[k] = -INFINITY; ti[k] = 0x7fffffff; }
+  for (int v = threadIdx.x; v < a.V; v += blockDim.x) {
+    float sv = ((lg[v] - mx) - lse) + bs;
+    const int f = fbase + v;
+    if (!beam_before(sv, f, tv[M - 1], ti[M - 1])) continue;
+    bool ban = false;
+    for (int k = 0; k < nbanned; ++k) ban = ban || (banned[k] == v);
+    if (ban) {
+      sv = -INFINITY;
+      if (!beam_before(sv, f, tv[M - 1], ti[M - 1])) continue;
+    }
+    bool placed = false;
+#pragma unroll
+    for (int k = M - 1; k > 0; --k) {
+      if (!placed) {
+        if (beam_before(sv, f, tv[k - 1], ti[k - 1])) { tv[k] = tv[k - 1]; ti[k] = ti[k - 1]; }
+        else { tv[k] = sv; ti[k] = f; placed = true; }
+      }
+    }
+    if (!placed) { tv[0] = sv; ti[0] = f; }
+  }
+  // pop the CTA's best head `need` times (flat indices are unique, so exactly one thread owns the winner)
+  for (int j = 0; j < need; ++j) {
+    float bv = tv[0];
+    int bi = ti[0];
+    for (int o = 16; o; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (beam_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    if (lane == 0) { win_v[j & 1][warp] = bv; win_i[j & 1][warp] = bi; }
+    __syncthreads();
+    bv = win_v[j & 1][0]; bi = win_i[j & 1][0];
+    for (int w = 1; w < nwarp; ++w)
+      if (beam_before(win_v[j & 1][w], win_i[j & 1][w], bv, bi)) { bv = win_v[j & 1][w]; bi = win_i[j & 1][w]; }
+    if (ti[0] == bi) {
+#pragma unroll
+      for (int k = 0; k < M - 1; ++k) { tv[k] = tv[k + 1]; ti[k] = ti[k + 1]; }
+      tv[M - 1] = -INFINITY; ti[M - 1] = 0x7fffffff;
+    }
+    if (threadIdx.x == 0) { co[j] = bv; ci[j] = bi; }
+  }
+}
+
+struct BeamUpdateArgs {
+  const float* cand_score; const int* cand_idx;   // [K * nb][2 nb], b2p_beam_topk
+  int V, nb;
+  int* seq; int seq_ld;                           // running sequences [K * nb][seq_ld]
+  int* src; int tmax;                             // cache ancestor table [K * nb][tmax]
+  const int* step;
+  int eos, pad, max_len, early_stopping, lp_positive;
+  const float* lp_pow;                            // [max_len + 1]: float(L ** length_penalty)
+  float* bscore; int* parent;                     // [K * nb]; parent: beam index of each new running row (may be null)
+  int* hyp_seq; float* hyp_score; int* hyp_len; int* hyp_fin;   // finished hypotheses [K * nb] (hyp_seq pitch seq_ld)
+  int* heur; int* done; int* n_open;              // [K], [K], counter of crops not done
+};
+
+// One CTA per crop: HF steps c-g.  Thread 0 makes the (small, serial) selections; the CTA stages the crop's seq / src rows in
+// shared memory and writes the parent-gathered rows back in place.
+__global__ void __launch_bounds__(256) beam_update_kernel(BeamUpdateArgs a) {
+  pdl_wait();
+  const int k = blockIdx.x, nb = a.nb, need = 2 * nb, r0 = k * nb;
+  if (a.done[k]) return;   // hypotheses are final (see include/b200parse.h): nothing of this crop changes any more
+  const int t = *a.step, cur_len = t + 1;   // the new token goes to position cur_len
+  extern __shared__ int bsm[];
+  int* sseq = bsm;                          // [nb][cur_len]
+  int* ssrc = bsm + nb * a.max_len;         // [nb][t]
+  __shared__ float top_s[2 * kBeamMax];
+  __shared__ int top_f[2 * kBeamMax];
+  __shared__ int run_from[kBeamMax];        // new running beam j <- top position
+  __shared__ float run_s[kBeamMax];
+  __shared__ int hyp_from[kBeamMax];        // new hypothesis slot j <- merged index (< nb: old slot, else nb + top position)
+  for (int i = threadIdx.x; i < nb * cur_len; i += blockDim.x) {
+    const int b = i / cur_len, j = i - b * cur_len;
+    sseq[i] = a.seq[(long long)(r0 + b) * a.seq_ld + j];
+  }
+  for (int i = threadIdx.x; i < nb * t; i += blockDim.x) {
+    const int b = i / t, j = i - b * t;
+    ssrc[i] = a.src[(long long)(r0 + b) * a.tmax + j];
+  }
+  if (threadIdx.x == 0) {
+    const float NEG = -1.0e9f;
+    // c. the crop's best 2 nb: merge of the rows' sorted lists
+    int head[kBeamMax];
+    for (int b = 0; b < nb; ++b) head[b] = 0;
+    for (int j = 0; j < need; ++j) {
+      int bb = -1, bi = 0;
+      float bv = 0.f;
+      for (int b = 0; b < nb; ++b) {
+        if (head[b] >= need) continue;
+        const float v = a.cand_score[(long long)(r0 + b) * need + head[b]];
+        const int f = a.cand_idx[(long long)(r0 + b) * need + head[b]];
+        if (bb < 0 || beam_before(v, f, bv, bi)) { bb = b; bv = v; bi = f; }
+      }
+      top_s[j] = bv; top_f[j] = bi; ++head[bb];
+    }
+    // d. stopping criteria per candidate: EOS, or the sequence reaches max_len
+    bool hit[2 * kBeamMax], all_hit = true;
+    for (int j = 0; j < need; ++j) {
+      hit[j] = (top_f[j] % a.V) == a.eos || cur_len + 1 >= a.max_len;
+      all_hit = all_hit && hit[j];
+    }
+    // e. running beams: best nb of score + hit * -1e9 (_get_running_beams_for_next_iteration)
+    float rs[2 * kBeamMax];
+    for (int j = 0; j < need; ++j) rs[j] = __fadd_rn(top_s[j], hit[j] ? NEG : -0.f);
+    unsigned used = 0;
+    for (int j = 0; j < nb; ++j) {
+      int bj = -1;
+      for (int i = 0; i < need; ++i)
+        if (!((used >> i) & 1u) && (bj < 0 || rs[i] > rs[bj])) bj = i;
+      used |= 1u << bj;
+      run_from[j] = bj; run_s[j] = rs[bj];
+    }
+    // f. finished hypotheses (_update_finished_beams), the same fp32 operations in the same order
+    const int h0 = r0;
+    bool all_fin = true;
+    for (int s = 0; s < nb; ++s) all_fin = all_fin && a.hyp_fin[h0 + s];
+    const bool heur = a.heur[k] != 0;
+    const float lpow = a.lp_pow[cur_len];
+    float c[2 * kBeamMax];
+    bool did[2 * kBeamMax];
+    for (int j = 0; j < need; ++j) {
+      float v = __fdiv_rn(top_s[j], lpow);
+      v = __fadd_rn(v, (all_fin && a.early_stopping == 1) ? NEG : -0.f);
+      v = __fadd_rn(v, heur ? -0.f : NEG);
+      did[j] = hit[j] && j < nb;
+      v = __fadd_rn(v, did[j] ? -0.f : NEG);
+      c[j] = v;
+    }
+    float old_s[kBeamMax], new_s[kBeamMax];
+    int old_f[kBeamMax], old_l[kBeamMax], new_f[kBeamMax];
+    for (int s = 0; s < nb; ++s) { old_s[s] = a.hyp_score[h0 + s]; old_f[s] = a.hyp_fin[h0 + s]; old_l[s] = a.hyp_len[h0 + s]; }
+    unsigned long long used2 = 0;
+    for (int j = 0; j < nb; ++j) {
+      int bj = -1;
+      float bv = 0.f;
+      for (int i = 0; i < nb + need; ++i) {
+        const float v = i < nb ? old_s[i] : c[i - nb];
+        if (!((used2 >> i) & 1ull) && (bj < 0 || v > bv)) { bj = i; bv = v; }
+      }
+      used2 |= 1ull << bj;
+      hyp_from[j] = bj;
+      new_s[j] = bv;
+      new_f[j] = bj < nb ? old_f[bj] : (int)did[bj - nb];
+      a.hyp_score[h0 + j] = bv;
+      a.hyp_fin[h0 + j] = new_f[j];
+      a.hyp_len[h0 + j] = bj < nb ? old_l[bj] : cur_len;
+    }
+    // g. early-stop heuristic at the next length (_check_early_stop_heuristic) and the crop's stopping condition
+    //    (_beam_search_has_unfinished_sequences restricted to this crop)
+    const int best_len = (a.early_stopping == 2 && a.lp_positive) ? a.max_len - 1 : cur_len;
+    const float best = __fdiv_rn(run_s[0], a.lp_pow[best_len]);
+    float mn = new_s[0];
+    for (int s = 1; s < nb; ++s) mn = fminf(mn, new_s[s]);
+    bool improvable = false, all_fin_new = true;
+    for (int s = 0; s < nb; ++s) {
+      improvable = improvable || best > (new_f[s] ? mn : NEG);
+      all_fin_new = all_fin_new && new_f[s];
+    }
+    const bool heur_new = heur && improvable;
+    a.heur[k] = heur_new;
+    const bool open = heur_new && !(all_fin_new && a.early_stopping == 1) && !all_hit;
+    if (!open) {
+      a.done[k] = 1;
+      if (a.n_open) atomicSub(a.n_open, 1);
+    }
+  }
+  __syncthreads();
+  // running rows: parent-gathered prefix + the new token; cache ancestors; scores
+  for (int i = threadIdx.x; i < nb * (cur_len + 1); i += blockDim.x) {
+    const int b = i / (cur_len + 1), j = i - b * (cur_len + 1);
+    const int f = top_f[run_from[b]], p = f / a.V;
+    a.seq[(long long)(r0 + b) * a.seq_ld + j] = j < cur_len ? sseq[p * cur_len + j] : f - p * a.V;
+  }
+  for (int i = threadIdx.x; i < nb * (t + 1); i += blockDim.x) {
+    const int b = i / (t + 1), j = i - b * (t + 1);
+    const int p = top_f[run_from[b]] / a.V;
+    a.src[(long long)(r0 + b) * a.tmax + j] = j < t ? ssrc[p * t + j] : r0 + p;
+  }
+  for (int b = threadIdx.x; b < nb; b += blockDim.x) {
+    a.bscore[r0 + b] = run_s[b];
+    if (a.parent) a.parent[r0 + b] = top_f[run_from[b]] / a.V;
+  }
+  // hypothesis rows, in place: the kept old slots are a prefix 0..m-1 of the old list and move to slots j >= their old
+  // index, so filling the slots from the last to the first never overwrites a row that is still to be read
+  for (int j = nb - 1; j >= 0; --j) {
+    const int from = hyp_from[j];
+    int* dst = a.hyp_seq + (long long)(r0 + j) * a.seq_ld;
+    if (from < nb) {
+      if (from != j) {
+        const int* srow = a.hyp_seq + (long long)(r0 + from) * a.seq_ld;
+        for (int i = threadIdx.x; i < a.seq_ld; i += blockDim.x) dst[i] = srow[i];
+      }
+    } else {
+      const int f = top_f[from - nb], p = f / a.V;
+      for (int i = threadIdx.x; i < a.seq_ld; i += blockDim.x)
+        dst[i] = i < cur_len ? sseq[p * cur_len + i] : (i == cur_len ? f - p * a.V : a.pad);
+    }
+    __syncthreads();
+  }
 }
 
 static inline int grid_for(long long n, int threads) {
@@ -899,7 +1209,7 @@ int b2p_mha(const float* q, long long ldq, const float* k, const float* v, long 
   a.B = B; a.Lq = Lq; a.Lk = Lk; a.heads = heads; a.out = (__half*)out; a.ldo = ldo; a.split = (split & 1) ? heads * 64 : 0;
   const int total = B * heads * Lq;
   // (a thread-per-query variant is slower here: its per-thread 256-B rows are uncoalesced)
-  launch_pdl(mha_kernel, dim3((total + 7) / 8), dim3(256), 0, st, a);
+  launch_pdl(mha_kernel<false>, dim3((total + 7) / 8), dim3(256), 0, st, a);
   B2P_CHECK_LAUNCH();
   return 0;
 }
@@ -913,7 +1223,7 @@ int b2p_mha_cached(const float* q, long long ldq, const float* knew, const float
   a.kcache = kcache; a.vcache = vcache; a.tmax = tmax; a.step = step;
   a.B = B; a.Lq = 1; a.Lk = 0; a.heads = heads; a.out = (__half*)out; a.ldo = ldo; a.split = split ? heads * 64 : 0;
   const int total = B * heads;
-  launch_pdl(mha_kernel, dim3((total + 7) / 8), dim3(256), 0, st, a);
+  launch_pdl(mha_kernel<false>, dim3((total + 7) / 8), dim3(256), 0, st, a);
   B2P_CHECK_LAUNCH();
   return 0;
 }
@@ -960,6 +1270,93 @@ int b2p_greedy_pick(const float* logits, long long ld, int V, int B, int* seq, i
 
 int b2p_step_advance(int* step, cudaStream_t st) {
   launch_pdl(step_advance_kernel, dim3(1), dim3(1), 0, st, step);
+  B2P_CHECK_LAUNCH();
+  return 0;
+}
+
+int b2p_mha_cached_beam(const float* q, long long ldq, const float* knew, const float* vnew, long long ldnew, float* kcache,
+                        float* vcache, int tmax, const int* step, const int* src, int B, int heads, void* out, long long ldo,
+                        int split, cudaStream_t st) {
+  if (B < 0) return set_error("mha_cached_beam: B must be >= 0");
+  if (B == 0) return 0;
+  if (!src || tmax < 1) return set_error("mha_cached_beam: needs the ancestor table src [B][tmax]");
+  MhaArgs a{};
+  a.q = q; a.ldq = ldq; a.knew = knew; a.vnew = vnew; a.ldnew = ldnew;
+  a.kcache = kcache; a.vcache = vcache; a.tmax = tmax; a.step = step; a.src = src;
+  a.B = B; a.Lq = 1; a.Lk = 0; a.heads = heads; a.out = (__half*)out; a.ldo = ldo; a.split = split ? heads * 64 : 0;
+  launch_pdl(mha_kernel<true>, dim3((B * heads + 7) / 8), dim3(256), 0, st, a);
+  B2P_CHECK_LAUNCH();
+  return 0;
+}
+
+int b2p_mha_grouped(const float* q, long long ldq, const float* k, const float* v, long long ldk, int B, int Lq, int Lk,
+                    int heads, int rows_per_kv, void* out, long long ldo, int split, cudaStream_t st) {
+  if (B < 0) return set_error("mha_grouped: B must be >= 0");
+  if (B == 0) return 0;
+  if (rows_per_kv < 1) return set_error("mha_grouped: rows_per_kv must be >= 1");
+  MhaArgs a{};
+  a.q = q; a.ldq = ldq; a.k = k; a.v = v; a.ldk = ldk; a.rows_per_kv = rows_per_kv;
+  a.B = B; a.Lq = Lq; a.Lk = Lk; a.heads = heads; a.out = (__half*)out; a.ldo = ldo; a.split = (split & 1) ? heads * 64 : 0;
+  launch_pdl(mha_kernel<true>, dim3((B * heads * Lq + 7) / 8), dim3(256), 0, st, a);
+  B2P_CHECK_LAUNCH();
+  return 0;
+}
+
+int b2p_beam_topk(const float* logits, long long ld, int V, int B, int nb, const int* seq, int seq_ld, const int* step,
+                  int ngram, int forced_bos, int forced_eos, int max_len, const float* bscore, const int* done,
+                  float* cand_score, int* cand_idx, cudaStream_t st) {
+  if (B < 0) return set_error("beam_topk: B must be >= 0");
+  if (nb < 1 || nb > kBeamMax) return set_error("beam_topk: num_beams must be in [1, 16]");
+  if (B % nb) return set_error("beam_topk: B must be a multiple of num_beams");
+  if (V < 2 * nb || ld < V) return set_error("beam_topk: need 2 * num_beams <= V <= ld");
+  if ((long long)V * nb > 0x7fffffffLL) return set_error("beam_topk: num_beams * V must fit in int");
+  if (ngram < 0) return set_error("beam_topk: ngram must be >= 0 (0 = no n-gram ban)");
+  if (max_len < 2 || max_len > kPickMaxLen) return set_error("beam_topk: max_len must be in [2, 8192]");
+  if (seq_ld < max_len) return set_error("beam_topk: seq_ld must be >= max_len");
+  if (forced_bos >= V || forced_eos >= V) return set_error("beam_topk: forced token ids must be < V");
+  if (B == 0) return 0;
+  BeamTopkArgs a{};
+  a.logits = logits; a.ld = ld; a.V = V; a.nb = nb; a.seq = seq; a.seq_ld = seq_ld; a.step = step;
+  a.ngram = ngram; a.forced_bos = forced_bos; a.forced_eos = forced_eos; a.max_len = max_len;
+  a.bscore = bscore; a.done = done; a.cand_score = cand_score; a.cand_idx = cand_idx;
+  const size_t smem = size_t(max_len) * sizeof(int);
+  if (nb <= 2) launch_pdl(beam_topk_kernel<4>, dim3(B), dim3(256), smem, st, a);
+  else if (nb <= 4) launch_pdl(beam_topk_kernel<8>, dim3(B), dim3(256), smem, st, a);
+  else if (nb <= 8) launch_pdl(beam_topk_kernel<16>, dim3(B), dim3(256), smem, st, a);
+  else launch_pdl(beam_topk_kernel<32>, dim3(B), dim3(256), smem, st, a);
+  B2P_CHECK_LAUNCH();
+  return 0;
+}
+
+int b2p_beam_update(const float* cand_score, const int* cand_idx, int V, int K, int nb, int* seq, int seq_ld, int* src,
+                    int tmax, const int* step, int eos, int pad, int max_len, int early_stopping, float length_penalty,
+                    const float* lp_pow, float* bscore, int* parent, int* hyp_seq, float* hyp_score, int* hyp_len,
+                    int* hyp_fin, int* heur, int* done, int* n_open, cudaStream_t st) {
+  if (K < 0) return set_error("beam_update: K must be >= 0");
+  if (nb < 1 || nb > kBeamMax) return set_error("beam_update: num_beams must be in [1, 16]");
+  if (V < 2 * nb) return set_error("beam_update: need 2 * num_beams <= V");
+  if ((long long)V * nb > 0x7fffffffLL) return set_error("beam_update: num_beams * V must fit in int");
+  if (max_len < 2 || max_len > kPickMaxLen) return set_error("beam_update: max_len must be in [2, 8192]");
+  if (seq_ld < max_len) return set_error("beam_update: seq_ld must be >= max_len");
+  if (tmax < max_len - 1) return set_error("beam_update: tmax must be >= max_len - 1");
+  if ((long long)nb * max_len > kBeamSeqInts) return set_error("beam_update: num_beams * max_len must be <= 16384");
+  if (early_stopping < 0 || early_stopping > 2) return set_error("beam_update: early_stopping must be 0 (False), 1 (True) or 2 (\"never\")");
+  if (!lp_pow) return set_error("beam_update: needs the length-penalty table lp_pow [max_len + 1]");
+  if (K == 0) return 0;
+  const size_t smem = size_t(2) * nb * max_len * sizeof(int);
+  static std::atomic<bool> attr{false};
+  if (!attr) {
+    if (int e = bind_device()) return e;
+    if (cudaFuncSetAttribute(beam_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(2 * kBeamSeqInts * sizeof(int))) != cudaSuccess)
+      return set_error("beam_update: cudaFuncSetAttribute failed");
+    attr = true;
+  }
+  BeamUpdateArgs a{};
+  a.cand_score = cand_score; a.cand_idx = cand_idx; a.V = V; a.nb = nb; a.seq = seq; a.seq_ld = seq_ld; a.src = src; a.tmax = tmax;
+  a.step = step; a.eos = eos; a.pad = pad; a.max_len = max_len; a.early_stopping = early_stopping; a.lp_positive = length_penalty > 0.f;
+  a.lp_pow = lp_pow; a.bscore = bscore; a.parent = parent; a.hyp_seq = hyp_seq; a.hyp_score = hyp_score; a.hyp_len = hyp_len;
+  a.hyp_fin = hyp_fin; a.heur = heur; a.done = done; a.n_open = n_open;
+  launch_pdl(beam_update_kernel, dim3(K), dim3(256), smem, st, a);
   B2P_CHECK_LAUNCH();
   return 0;
 }

@@ -171,11 +171,20 @@ class FlorencePlan:
     D = 768
     HEADS = 12
 
-    def __init__(self, w: FlorenceWeights, K: int, max_new_tokens: int, prompt_ids: List[int], use_graph=True, size: int = 64, instance: int = 0):
+    def __init__(self, w: FlorenceWeights, K: int, max_new_tokens: int, prompt_ids: List[int], use_graph=True, size: int = 64, instance: int = 0,
+                 *, num_beams: int = 1, early_stopping=True, length_penalty: float = 1.0):
         """instance: plans of different instances own disjoint buffers and capture streams (split-K scratch is keyed by
         stream), so they may run concurrently on different streams.  size = 64: the reference's CUDA branch (crops fed un-resized, 5 image tokens, ref:util/utils.py:121);
-        size = 768: its CPU branch (CLIP processor bicubic resize of every crop to 768x768, 577 image tokens, :123)."""
+        size = 768: its CPU branch (CLIP processor bicubic resize of every crop to 768x768, 577 image tokens, :123).
+        num_beams > 1: HF beam search (early_stopping True / False / "never", length_penalty); the encoder runs on the K crops,
+        the decoder on K * num_beams rows (see _build_dec_part)."""
         assert size in (64, 768)
+        if not 1 <= num_beams <= 16:
+            raise ValueError(f"num_beams must be in [1, 16], got {num_beams}")
+        if not (early_stopping is True or early_stopping is False or early_stopping == "never"):
+            raise ValueError(f"early_stopping must be True, False or 'never', got {early_stopping!r}")
+        self.nb = num_beams
+        self.early_stopping, self.length_penalty = early_stopping, float(length_penalty)
         self.S = size
         self.tag = f"florence{instance}"
         # smem-tiled dwconv+LN and warp-per-group channel attention (N <= 16): bit-identical with the per-token / per-CTA kernels
@@ -204,10 +213,11 @@ class FlorencePlan:
         self.n_prompt = len(prompt_ids)
         self.n_img = (size // 32) ** 2 + 1
         self.L = self.n_img + self.n_prompt
-        self.seq = torch.zeros((K, self.max_len + 1), dtype=torch.int32, device=dev)
+        self.R = R = K * self.nb            # decoder rows: crop * num_beams + beam
+        self.seq = torch.zeros((R, self.max_len + 1), dtype=torch.int32, device=dev)
         self.finished = torch.zeros((K,), dtype=torch.int32, device=dev)
         # row pitch padded to 8 floats so the LM-head epilogue takes the 16-byte vector store path (51290 is not)
-        self._logits_buf = torch.zeros((K, (w.vocab + 7) // 8 * 8), dtype=torch.float32, device=dev)
+        self._logits_buf = torch.zeros((R, (w.vocab + 7) // 8 * 8), dtype=torch.float32, device=dev)
         self.logits = self._logits_buf[:, :w.vocab]
         self.enc_ops, self.dec_ops = [], []
         self._pools = {}
@@ -395,6 +405,12 @@ class FlorencePlan:
         (every chain re-streams the 0.5 GB of decoder weights), so the default is one chain."""
         K = self.K
         P = int(os.environ.get("B2P_DECODE_PARTS", "1"))   # more chains: the weights stream once per chain
+        if self.nb > 1:
+            if P > 1:
+                raise ValueError("B2P_DECODE_PARTS > 1 is not supported with beam search (num_beams > 1)")
+            self.parts = [self._build_dec_part(0, 0, self.R)]
+            self.dec_ops = list(self.parts[0]["ops"])
+            return
         if K < 64 * P:
             P = 1
         per = (K // P + 15) // 16 * 16 if P > 1 else K
@@ -414,7 +430,10 @@ class FlorencePlan:
         ops_ = []
         seq, finished, logits = self.seq[r0:r1], self.finished[r0:r1], self.logits[r0:r1]
         step = torch.zeros((1,), dtype=torch.int32, device=self.dev)
-        n_unf = torch.zeros((1,), dtype=torch.int32, device=self.dev)
+        n_unf = torch.zeros((1,), dtype=torch.int32, device=self.dev)   # beam search: crops not done
+        nb = self.nb
+        if nb > 1:
+            self._alloc_beam_state(tmax)
         e0 = self._e(R, D)
         ops_.append(lambda: ops.decoder_embed(w.E32, seq, seq.stride(0), step, w.dec_pos, R, D, e0))
         x = self._e(R, D); h = self._act(R, D)
@@ -425,8 +444,12 @@ class FlorencePlan:
             kc = torch.zeros((R, tmax, D), dtype=torch.float32, device=self.dev)
             vc = torch.zeros((R, tmax, D), dtype=torch.float32, device=self.dev)
             a = self._act(R, D)
-            ops_.append(lambda qkv=qkv, kc=kc, vc=vc, a=a: ops.mha_cached(qkv, 3 * D, qkv[:, D:], qkv[:, 2 * D:], 3 * D, kc, vc, tmax,
-                                                                       step, R, self.HEADS, a, a.stride(0), split=x3))
+            if nb > 1:   # beam-indexed cache: a beam reorder rewrites self.src, never the caches
+                ops_.append(lambda qkv=qkv, kc=kc, vc=vc, a=a: ops.mha_cached_beam(qkv, 3 * D, qkv[:, D:], qkv[:, 2 * D:], 3 * D, kc, vc,
+                                                                                tmax, step, self.src, R, self.HEADS, a, a.stride(0), split=x3))
+            else:
+                ops_.append(lambda qkv=qkv, kc=kc, vc=vc, a=a: ops.mha_cached(qkv, 3 * D, qkv[:, D:], qkv[:, 2 * D:], 3 * D, kc, vc, tmax,
+                                                                           step, R, self.HEADS, a, a.stride(0), split=x3))
             if self.fuse_ln:
                 xn = self._e(R, D); h = self._act(R, D)
                 self._gemm_ln(ops_, a, lay["o"], x, lay["ln1"], h, xn)
@@ -438,9 +461,14 @@ class FlorencePlan:
                 self._ln(ops_, y, lay["ln1"], R, D, h, x)
             q = self._e(R, D)
             self._gemm(ops_, h, lay["cq"], q, enc=False)
-            kv = self.cross_kv[li][r0 * self.L:r1 * self.L]
             a2 = self._act(R, D)
-            ops_.append(lambda q=q, kv=kv, a2=a2: ops.mha(q, D, kv, kv[:, D:], 2 * D, R, 1, self.L, self.HEADS, a2, a2.stride(0), split=x3))
+            if nb > 1:   # the nb beams of a crop share its cross K / V
+                kv = self.cross_kv[li]
+                ops_.append(lambda q=q, kv=kv, a2=a2: ops.mha_grouped(q, D, kv, kv[:, D:], 2 * D, R, 1, self.L, self.HEADS, nb, a2,
+                                                                      a2.stride(0), split=x3))
+            else:
+                kv = self.cross_kv[li][r0 * self.L:r1 * self.L]
+                ops_.append(lambda q=q, kv=kv, a2=a2: ops.mha(q, D, kv, kv[:, D:], 2 * D, R, 1, self.L, self.HEADS, a2, a2.stride(0), split=x3))
             if self.fuse_ln:
                 xn = self._e(R, D); h = self._act(R, D)
                 self._gemm_ln(ops_, a2, lay["co"], x, lay["ln2"], h, xn)
@@ -466,17 +494,58 @@ class FlorencePlan:
         self._gemm(ops_, h, lm, logits, enc=False)
         fb = g.get("forced_bos_token_id")
         fe = g.get("forced_eos_token_id")
-        pick = lambda dump=None: ops.greedy_pick(logits, logits.stride(0), w.vocab, R, seq, seq.stride(0), finished, step,
-                                                 g.get("no_repeat_ngram_size", 0) or 0, -1 if fb is None else fb,
-                                                 -1 if fe is None else fe, g["eos_token_id"], g["pad_token_id"], self.max_len,
-                                                 dump, n_unf)
+        ngram = g.get("no_repeat_ngram_size", 0) or 0
+        fb, fe = -1 if fb is None else fb, -1 if fe is None else fe
+        if nb > 1:
+            es = {False: 0, True: 1, "never": 2}[self.early_stopping]
+            pick = None
+            pick_ops = [lambda: ops.beam_topk(logits, logits.stride(0), w.vocab, R, nb, seq, seq.stride(0), step, ngram, fb, fe,
+                                              self.max_len, self.bscore, self.done, self.cand_score, self.cand_idx),
+                        lambda: ops.beam_update(self.cand_score, self.cand_idx, w.vocab, self.K, nb, seq, seq.stride(0), self.src, tmax,
+                                                step, g["eos_token_id"], g["pad_token_id"], self.max_len, es, self.length_penalty,
+                                                self.lp_pow, self.bscore, self.parent, self.hyp_seq, self.hyp_score, self.hyp_len,
+                                                self.hyp_fin, self.heur, self.done, n_unf)]
+        else:
+            pick = lambda dump=None: ops.greedy_pick(logits, logits.stride(0), w.vocab, R, seq, seq.stride(0), finished, step, ngram,
+                                                     fb, fe, g["eos_token_id"], g["pad_token_id"], self.max_len, dump, n_unf)
+            pick_ops = [lambda: pick(None)]
         # Steps whose token is forced by the generation config (forced BOS at length 1, forced EOS at the last length:
         # hf:generation/logits_process.py:1552,1597) never look at the logits: the pick kernel writes the forced id without
         # reading them, so those steps replay a graph WITHOUT the LM head (51290 x 768, the largest GEMM of the step).  The
         # decoder layers still run: the KV cache of the step is needed by the following steps.
         return dict(idx=idx, r0=r0, r1=r1, ops=ops_, pick=pick, step=step, n_unf=n_unf, graph=None, graph_forced=None,
-                    stream=torch.cuda.Stream(device=self.dev), full=ops_ + [lambda: pick(None), lambda: ops.step_advance(step)],
-                    full_forced=ops_[:-1] + [lambda: pick(None), lambda: ops.step_advance(step)])
+                    stream=torch.cuda.Stream(device=self.dev), full=ops_ + pick_ops + [lambda: ops.step_advance(step)],
+                    full_forced=ops_[:-1] + pick_ops + [lambda: ops.step_advance(step)])
+
+    def _alloc_beam_state(self, tmax):
+        """Beam-search state (b2p_beam_topk / b2p_beam_update): running scores, cache ancestor table, candidates, finished
+        hypotheses (HF's `sequences` / `beam_scores` / `is_sent_finished`), per-crop heuristic and done flags."""
+        R, K, nb, dev = self.R, self.K, self.nb, self.dev
+        if nb * self.max_len > 16384:
+            raise ValueError(f"num_beams * (max_new_tokens + 1) = {nb * self.max_len} exceeds 16384 (beam state staged in shared memory)")
+        self.bscore = self._e(R)
+        self.parent = torch.zeros((R,), dtype=torch.int32, device=dev)
+        self.src_init = torch.arange(R, dtype=torch.int32, device=dev)[:, None].expand(R, tmax).contiguous()
+        self.src = self.src_init.clone()
+        self.cand_score = self._e(R, 2 * nb)
+        self.cand_idx = torch.zeros((R, 2 * nb), dtype=torch.int32, device=dev)
+        self.hyp_seq = torch.zeros((R, self.max_len + 1), dtype=torch.int32, device=dev)
+        self.hyp_score = self._e(R)
+        self.hyp_len = torch.zeros((R,), dtype=torch.int32, device=dev)
+        self.hyp_fin = torch.zeros((R,), dtype=torch.int32, device=dev)
+        self.heur = torch.zeros((K,), dtype=torch.int32, device=dev)
+        self.done = torch.zeros((K,), dtype=torch.int32, device=dev)
+        # float(L ** length_penalty) in double, rounded once: what torch's fp32-tensor / Python-float division uses
+        lp = self.length_penalty
+        self.lp_pow = torch.tensor([1.0] + [float(L) ** lp for L in range(1, self.max_len + 1)], dtype=torch.float32).to(dev)
+
+    def beam_sequences(self, n: int, num_return_sequences: int = 1) -> torch.Tensor:
+        """HF's beam-search output for the first n crops: [n * num_return_sequences, 1 + longest returned hypothesis],
+        best first within each crop, pad-filled (hf:generation/utils.py:3370-3386)."""
+        nrs = num_return_sequences
+        hs = self.hyp_seq.view(self.K, self.nb, -1)[:n, :nrs]
+        width = 1 + int(self.hyp_len.view(self.K, self.nb)[:n, :nrs].max().item()) if n else 1
+        return hs[:, :, :width].reshape(n * nrs, width).long()
 
     # ------------------------------------------------------------------ running
     def _run(self, lst, holder, key, tag, replay_after_capture=True):
@@ -547,6 +616,17 @@ class FlorencePlan:
         self.finished.zero_()
         if n_active < self.K:
             self.finished[n_active:] = 1     # padding rows never gate the stop test
+        if self.nb > 1:                      # hf:generation/utils.py:3193-3205
+            self.bscore.view(self.K, self.nb).fill_(-1.0e9)
+            self.bscore.view(self.K, self.nb)[:, 0] = 0.0
+            self.src.copy_(self.src_init)
+            self.hyp_seq.fill_(self.w.gen["pad_token_id"])
+            self.hyp_score.fill_(-1.0e9)
+            self.hyp_len.zero_()
+            self.hyp_fin.zero_()
+            self.heur.fill_(1)
+            self.done.zero_()
+            self.done[n_active:] = 1         # padding crops are never decoded into hypotheses
         for pt in self.parts:
             pt["step"].zero_()
             pt["n_unf"].fill_(max(0, min(n_active, pt["r1"]) - pt["r0"]))
@@ -584,6 +664,8 @@ class FlorencePlan:
                 with torch.cuda.stream(pt["stream"]):
                     self._run(pt[lst], pt, key, f"{self.tag}_dec{pt['idx']}", replay_after_capture=False)
             return
+        if self.nb > 1:
+            raise NotImplementedError("dump / teacher forcing are greedy-plan tools (num_beams == 1)")
         for pt in self.parts:   # eager path used by the parity tests
             for f in pt["ops"]:
                 f()

@@ -301,3 +301,28 @@ def greedy_pick(logits, ld, V, B, seq, seq_ld, finished, step, ngram, forced_bos
 
 def step_advance(step):
     _lib.check(_lib.lib().b2p_step_advance(_p(step), _stream()))
+
+
+# beam search (include/b200parse.h): rows r = crop * nb + beam; early_stopping 0 = False, 1 = True, 2 = "never"
+def beam_topk(logits, ld, V, B, nb, seq, seq_ld, step, ngram, forced_bos, forced_eos, max_len, bscore, done, cand_score,
+              cand_idx):
+    _lib.check(_lib.lib().b2p_beam_topk(_p(logits), ld, V, B, nb, _p(seq), seq_ld, _p(step), ngram, forced_bos, forced_eos,
+                                        max_len, _p(bscore), _p(done), _p(cand_score), _p(cand_idx), _stream()))
+
+
+def beam_update(cand_score, cand_idx, V, K, nb, seq, seq_ld, src, tmax, step, eos, pad, max_len, early_stopping,
+                length_penalty, lp_pow, bscore, parent, hyp_seq, hyp_score, hyp_len, hyp_fin, heur, done, n_open):
+    _lib.check(_lib.lib().b2p_beam_update(_p(cand_score), _p(cand_idx), V, K, nb, _p(seq), seq_ld, _p(src), tmax, _p(step), eos,
+                                          pad, max_len, early_stopping, float(length_penalty), _p(lp_pow), _p(bscore),
+                                          _p(parent), _p(hyp_seq), _p(hyp_score), _p(hyp_len), _p(hyp_fin), _p(heur), _p(done),
+                                          _p(n_open), _stream()))
+
+
+def mha_cached_beam(q, ldq, knew, vnew, ldnew, kcache, vcache, tmax, step, src, B, heads, out, ldo, split=False):
+    _lib.check(_lib.lib().b2p_mha_cached_beam(_p(q), ldq, _p(knew), _p(vnew), ldnew, _p(kcache), _p(vcache), tmax, _p(step),
+                                              _p(src), B, heads, _p(out), ldo, int(split), _stream()))
+
+
+def mha_grouped(q, ldq, k, v, ldk, B, Lq, Lk, heads, rows_per_kv, out, ldo, split=False):
+    _lib.check(_lib.lib().b2p_mha_grouped(_p(q), ldq, _p(k), _p(v), ldk, B, Lq, Lk, heads, rows_per_kv, _p(out), ldo,
+                                          int(bool(split)), _stream()))

@@ -22,8 +22,8 @@ import torch
 from PIL import Image
 
 from . import host_glue, ops, som_overlay
-from .caption import (CAPTION_PROMPT_IDS, B200Florence2Model, B200Florence2Processor, find_tokenizer_dir, load_florence_state,
-                      load_tokenizer)
+from .caption import (CAPTION_PROMPT_IDS, B200Florence2Model, B200Florence2Processor, beam_settings, find_tokenizer_dir,
+                      load_beam_defaults, load_florence_state, load_tokenizer)
 from .detector import B200YOLOv9Detector
 
 
@@ -61,7 +61,8 @@ def get_caption_model_processor(model_name, model_name_or_path="microsoft/Floren
             "(allow_id_captions=True returns token-id tags instead of strings)")
     sd, gen = load_florence_state(model_name_or_path)
     tok = load_tokenizer(tdir) if tdir is not None else None
-    model = B200Florence2Model(sd, device, gen, precision, name_or_path=str(model_name_or_path))
+    model = B200Florence2Model(sd, device, gen, precision, name_or_path=str(model_name_or_path),
+                               beam_defaults=load_beam_defaults(model_name_or_path))
     if "florence" not in model.config.name_or_path.lower():
         model.config.name_or_path = "florence2:" + model.config.name_or_path   # ref:util/utils.py:109 looks for 'florence'
     return {"model": model, "processor": B200Florence2Processor(tok)}
@@ -91,12 +92,17 @@ def _check_crop_status(status: torch.Tensor) -> None:
 def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, caption_model_processor: dict,
                       ocr: Sequence[tuple], BOX_TRESHOLD=0.01, iou_threshold=0.9, imgsz=640, max_new_tokens=20,
                       prompt_ids: Sequence[int] = CAPTION_PROMPT_IDS, timings: Optional[ParseTimings] = None,
-                      _skip_h2d: bool = False, _det_override=None, caption_size: int = 64):
+                      _skip_h2d: bool = False, _det_override=None, caption_size: int = 64, num_beams: int = 1,
+                      early_stopping=None, length_penalty=None):
     """``caption_size`` 64 = the reference's CUDA branch (crops captioned at 64x64, ref:util/utils.py:121); 768 = its
     CPU branch (CLIP processor bicubic-resizes every crop to 768x768 first, :123), done on the device, in chunks.
     Same-size u8 HWC screenshots + per-image ``(ocr_text, ocr_bbox_xyxy_pixels)`` -> per-image
     ``(filtered_boxes_elem, caption_token_ids)``; the compute of ``get_som_labeled_img`` without the overlay drawing.
-    NMS IoU is fixed at 0.1 as in ref:util/utils.py:431; ``iou_threshold`` feeds the overlap filter (:446)."""
+    NMS IoU is fixed at 0.1 as in ref:util/utils.py:431; ``iou_threshold`` feeds the overlap filter (:446).
+    ``num_beams`` > 1 captions with HF beam search (one caption per crop; early_stopping / length_penalty default to the
+    caption model's ``beam_defaults``)."""
+    bs = beam_settings(num_beams, False, early_stopping, length_penalty, 1, caption_model_processor["model"].beam_defaults)
+    bs.pop("num_return_sequences")
     B = len(images)
     H, W = images[0].shape[:2]
     cap_model: B200Florence2Model = caption_model_processor["model"]
@@ -145,7 +151,7 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
           with cap_model._lock:   # plan instance 0 of the caption handle (also what model.generate() uses)
             dev = model.device
             if caption_size == 64:
-                plan = cap_model.plan_for(n, max_new_tokens, prompt_ids)
+                plan = cap_model.plan_for(n, max_new_tokens, prompt_ids, **bs)
                 crops_dst = plan.crops
             else:
                 crops_dst = torch.empty((n, 64, 64, 3), dtype=torch.uint8, device=dev)
@@ -165,7 +171,7 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
             if caption_size == 64:
                 ids = cap_model.generate_from_device_crops(plan, n).cpu()  # D2H #2 (sync)
             else:
-                ids = cap_model.generate_chunked(crops_dst, max_new_tokens, prompt_ids, from_resized=False).cpu()
+                ids = cap_model.generate_chunked(crops_dst, max_new_tokens, prompt_ids, from_resized=False, **bs).cpu()
             _check_crop_status(status)
         t3 = time.perf_counter()
     out = []
