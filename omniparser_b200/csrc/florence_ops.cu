@@ -395,7 +395,12 @@ __global__ void window_attn_kernel(const float* __restrict__ qkv, const float* _
 // ---------------------------------------------------------------------------------------- channel attention
 // hf:models/florence2/modeling_florence2.py:228-264: per (batch, group) a d x d (d = 32) attention over channels:
 // S[i][j] = N^-0.5 * sum_n q[n][i] k[n][j]; P = softmax_j(S); out[n][i] = sum_j P[i][j] v[n][j].
-// One CTA (1024 threads = 32 x 32) per (batch, group); tokens streamed through shared memory in chunks.
+// One CTA (256 threads = 8 warps x 32 columns) per (batch, group); tokens streamed through shared memory in chunks.
+// Each chunk's 64 products are summed in fp32 into a fresh register and the chunk sums are added in fp64, in chunk order.
+// One fp32 running sum over all N tokens lost ~eps * N^1.5 when the inputs have a non-zero mean (they are a biased linear
+// layer's output): at the 768 mode's 36 864 tokens the [hi | lo] outputs were 21x over their 2e-5 bound
+// (tests/test_davit_kernels_gpu.py).  N <= 64 is one chunk: the same sums as before, so channel_attn_small_kernel stays
+// bit-identical with this kernel (float(double(s) * sc) is the fp32 product s * sc).
 __global__ void __launch_bounds__(256) channel_attn_kernel(const float* __restrict__ qkv, int N, int C, int groups,
                                                            __half* __restrict__ out, int split) {
   pdl_wait();   // PDL: inputs come from the previous kernel in the stream
@@ -405,7 +410,7 @@ __global__ void __launch_bounds__(256) channel_attn_kernel(const float* __restri
   const int g = blockIdx.x % groups, b = blockIdx.x / groups;
   const int w = threadIdx.x >> 5, j = threadIdx.x & 31;   // warp w owns rows i = 4w .. 4w+3, lane = column j
   const float* base = qkv + (long long)b * N * 3 * C;
-  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  double s[4] = {0.0, 0.0, 0.0, 0.0};
   for (int n0 = 0; n0 < N; n0 += CH) {
     const int cn = min(CH, N - n0);
     for (int t = threadIdx.x; t < cn * D; t += blockDim.x) {
@@ -414,17 +419,20 @@ __global__ void __launch_bounds__(256) channel_attn_kernel(const float* __restri
       ks[n][d] = base[(long long)(n0 + n) * 3 * C + C + g * D + d];
     }
     __syncthreads();
+    float cs[4] = {0.f, 0.f, 0.f, 0.f};
     for (int n = 0; n < cn; ++n) {
       const float kv = ks[n][j];
 #pragma unroll
-      for (int r = 0; r < 4; ++r) s[r] += qs[n][4 * w + r] * kv;
+      for (int r = 0; r < 4; ++r) cs[r] += qs[n][4 * w + r] * kv;
     }
+#pragma unroll
+    for (int r = 0; r < 4; ++r) s[r] += double(cs[r]);
     __syncthreads();
   }
   const float sc = rsqrtf(float(N));
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
-    const float v = s[r] * sc;
+    const float v = float(s[r] * double(sc));
     const float m = warp_max(v);
     const float e = __expf(v - m);
     P[4 * w + r][j] = e / warp_sum(e);

@@ -129,9 +129,10 @@ def test_768_mode_encoder_logits_and_ids(setup768):
     e_enc = (plan.enc_out32.view(K768, 585, 768).cpu() - out.encoder_last_hidden_state).abs().max().item()
     print(f"[768] image tokens max abs err {e_img:.5f} (|ref| max {img.abs().max():.2f}); encoder states max abs err {e_enc:.5f} "
           f"(|ref| max {out.encoder_last_hidden_state.abs().max():.2f})")
-    # 36864 stage-0 tokens per crop: fp32 summation-order differences in the channel attention / LN accumulate a little
-    # more than in the 64x64 mode (1e-3 there); the logits bound below is the north-star tolerance and is unchanged
-    assert e_img < 5e-3 and e_enc < 5e-3
+    # the 64x64 mode's bound.  It was 5e-3 while channel_attn_kernel summed 36864 stage-0 tokens in one fp32 running sum:
+    # 2.6e-3 / 8.2e-4 then, 1.3e-4 / 7e-5 with chunk sums added in fp64 (one H100 80GB HBM3, 700 W power limit); the
+    # kernel's own bound is tested in tests/test_davit_kernels_gpu.py
+    assert e_img < 1e-3 and e_enc < 1e-3
     plan.reset_decode(K768)
     dump = torch.empty((K768, w.vocab), dtype=torch.float32, device=DEV)
     worst = 0.0

@@ -443,7 +443,9 @@ def test_window_attn_v3_equals_first_version_and_torch(B, H, C, heads, split):
 @pytest.mark.parametrize("split", [False, True])
 def test_window_attn_multi_window_maps_v3_flag(B, H, C, heads, split):
     """maps larger than one 12x12 window (16x16 in the 64x64-crop mode: windows of 144 / 48 / 48 / 16 real tokens) are not
-    covered by the one-window kernel: with the v3 flag the call must fall through to the per-window kernel, same results."""
+    covered by the one-window kernel: with the v3 flag the call must fall through to the per-window kernel, same results,
+    and both must match fp64 windowed attention with bias-padded windows."""
+    from test_davit_kernels_gpu import window_attn_ref
     g = torch.Generator().manual_seed(B * H + C + 5)
     qkv = torch.randn(B * H * H, 3 * C, generator=g).to(DEV)
     bias = torch.randn(3 * C, generator=g).to(DEV)
@@ -454,6 +456,10 @@ def test_window_attn_multi_window_maps_v3_flag(B, H, C, heads, split):
         torch.cuda.synchronize()
         outs.append(o)
     _act_close(outs[1], outs[0], C, split)
+    ref = window_attn_ref(qkv.cpu(), bias.cpu(), B, H, H, C, heads)
+    tol = (2e-5 if split else 1.5e-3) * max(1.0, ref.abs().max().item())
+    for o in outs:
+        assert (_pair_val(o.cpu(), C, split) - ref).abs().max().item() < tol
 
 
 @pytest.mark.parametrize("B,N,C", [(7, 16, 512), (5, 4, 1024), (3, 9, 256), (3, 64, 256), (2, 256, 128), (2, 100, 128)])
