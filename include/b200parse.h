@@ -59,6 +59,26 @@ int b2p_conv3x3_planes(const void* in, long long ld_in, int batch, int H, int W,
                        int Cout, void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act,
                        int flags, long long lo_a, long long lo_out, long long lo_res, b2p_stream_t stream);
 
+/* Host only (no device is touched): the plan the launch of b2p_conv3x3_planes (stride 1 | 2) or of b2p_gemm_planes
+ * (stride 0, with M = batch and K = Cin; H and W ignored) would make on a device with num_sms SMs and max_smem bytes of
+ * opt-in shared memory per block, under the same B2P_* environment knobs; flags as there, plus bit5: the park-only GEMM of
+ * b2p_gemm_ln.  Makes every host-side rejection the launch makes.  It assumes the launching stream owns a split-K workspace
+ * slot: a launch on a stream that finds all 24 slots taken by other streams is planned without split-K instead (and a
+ * park-only one is refused); b2p_gemm_last_plan tells what was launched.  plan_host receives 45 ints:
+ *   0 mode (0 GEMM, 1 conv s1 per tap, 2 conv s2 parity view, 3 conv s1 halo tile), 1 bk, 2 bn, 3 ksplit, 4 kb_per,
+ *   5 kb_merge, 6 stages, 7 stagesA, 8 sep, 9 bres, 10 nb, 11 tw, 12 tw_valid, 13 th, 14 m_tiles, 15 n_tiles, 16 mt_fast,
+ *   17 grid, 18 smem (bytes), 19 vec_ok, 20 split (lo-plane offset of the output, 0 = none), 21 res_lo, 22 park,
+ *   23 x3, 24 num_kb, 25 taps, 26 a_bytes, 27 a_slot, 28 b_bytes, 29 b_slot, 30 tiles_x, 31 tiles_y,
+ *   32 rank of A's tensor map, 33-37 its box (elements, unused dims 0), 38-39 B's box,
+ *   40 / 41 elements from A / B to one past the last element their tensor maps can address (saturating at 2^31-1),
+ *   42 / 43 swizzle span (bytes) of A's / B's tensor map, 44 swizzle span of the wgmma shared-memory descriptors.
+ * kb_per, num_kb and bk count the 32- or 64-wide k-blocks the kernel streams (halo mode: channel blocks of nine taps). */
+int b2p_gemm_plan(const void* in, long long ld_in, int batch, int H, int W, int Cin, int stride, const void* weight, int Cout,
+                  void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act, int flags,
+                  long long lo_a, long long lo_out, long long lo_res, int num_sms, int max_smem, int* plan_host);
+/* Host only: the same 45 fields for the most recent GEMM/conv launch made by the calling thread (-1 if it made none). */
+int b2p_gemm_last_plan(int* plan_host);
+
 /* ---- YOLOv9-E graph helpers (inside the TorchScript archive, ref:util/yolov9.py:120-121) ----
  * `_x3` forms: every map is an fp16 hi/lo pair (lo plane `lo*` elements after the hi plane, 0 = plain fp16); the
  * arithmetic runs on the exact fp32 sums hi + lo and the result is re-split. */

@@ -803,13 +803,13 @@ static EncodeTiledFn get_encode() {
 }
 
 static int encode(CUtensorMap* m, int bf16, int rank, const void* base, const cuuint64_t* dims,
-                  const cuuint64_t* strides_bytes, const cuuint32_t* box, int bk) {
+                  const cuuint64_t* strides_bytes, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn fn = get_encode();
   if (!fn) return set_error("cuTensorMapEncodeTiled entry point unavailable");
   cuuint32_t es[5] = {1, 1, 1, 1, 1};
   CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank,
                   const_cast<void*>(base), dims, strides_bytes, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                  swizzle,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char buf[256];
@@ -885,17 +885,44 @@ static int device_setup() {
 }
 
 
+// Environment knobs of the planner, read once per process by gemm_knobs(); plan_gemm() itself never reads the environment.
+struct GemmKnobs {
+  bool no_halo;       // B2P_NO_HALO: stride-1 convs use the per-tap path (mode 1) instead of the halo tile (mode 3)
+  bool no_halo32;     // B2P_NO_HALO32: no halo tile at 32-wide k-blocks
+  bool no_bres;       // B2P_NO_BRES: never keep the weights resident
+  bool no_split;      // B2P_NO_SPLITK: never split K
+  bool sk_last;       // B2P_SPLITK_LAST: split-K reduced by the last arriving CTA instead of the distributed reduction
+  bool few_ctas;      // unset B2P_DENSE_GRIDS: single-wave launches pay a charge per occupied SM
+  double cta_penalty; // B2P_CTA_PENALTY: microseconds charged per CTA (default 0.02)
+  int max_grid;       // B2P_MAX_GRID: experiment, cap the grid of launches that do not split K (0 = none)
+};
+static const GemmKnobs& gemm_knobs() {
+  static const GemmKnobs k = [] {
+    GemmKnobs v{};
+    v.no_halo = getenv("B2P_NO_HALO") != nullptr;
+    v.no_halo32 = getenv("B2P_NO_HALO32") != nullptr;
+    v.no_bres = getenv("B2P_NO_BRES") != nullptr;
+    v.no_split = getenv("B2P_NO_SPLITK") != nullptr;
+    v.sk_last = getenv("B2P_SPLITK_LAST") != nullptr;
+    v.few_ctas = getenv("B2P_DENSE_GRIDS") == nullptr;
+    v.cta_penalty = getenv("B2P_CTA_PENALTY") ? atof(getenv("B2P_CTA_PENALTY")) : 0.02;
+    v.max_grid = getenv("B2P_MAX_GRID") ? atoi(getenv("B2P_MAX_GRID")) : 0;
+    return v;
+  }();
+  return k;
+}
+
 // Choose the N tile and the split-K factor with a small time model (microseconds per CTA):
 //   per k-block  max(MMA issue, smem fill): MMA = 128 * bn * bk MACs at 2048 fp16 MACs per clock and SM, ~1.7 GHz under
 //   load; fill = (A + B bytes) at ~40 GB/s per SM (the L2's ~5.5 TB/s shared by 132 SMs)
 //   per item     ~2.5 us pipeline fill/drain + epilogue (~0.012 us per output column) + split-K park/reduce.
 // The constants are estimates from the H100 data sheet, not fitted to measurements.
 static void pick_tiling(int N, int m_tiles, int num_kb, int bk, uint32_t a_bytes, int bn_max, bool allow_split, bool x3,
-                        int* bn_out, int* ksplit_out) {
+                        int num_sms, int max_smem, const GemmKnobs& kn, int* bn_out, int* ksplit_out) {
   // single-wave launches: a charge per occupied SM (B2P_DENSE_GRIDS=1 selects the model that spreads every launch over as
-  // many SMs as it can; B2P_CTA_PENALTY = microseconds charged per CTA, default 0.02)
-  static const bool few_ctas = getenv("B2P_DENSE_GRIDS") == nullptr;
-  static const double cta_penalty = getenv("B2P_CTA_PENALTY") ? atof(getenv("B2P_CTA_PENALTY")) : 0.02;
+  // many SMs as it can)
+  const bool few_ctas = kn.few_ctas;
+  const double cta_penalty = kn.cta_penalty;
   const int n16 = (N + 15) / 16 * 16;
   double best_cost = -1;
   int best = 16, best_ks = 1;
@@ -911,11 +938,11 @@ static void pick_tiling(int N, int m_tiles, int num_kb, int bk, uint32_t a_bytes
     // fp16x3 operands: three MMAs and two (hi, lo) tile pairs per logical k-block
     const double t_mma = (x3 ? 3.0 : 1.0) * double(c) * bk / 16.0 / 1700.0;
     const double t_fill = (x3 ? 2.0 : 1.0) * (double(a_bytes) + double(c) * bk * 2.0) / 40000.0;
-    if (x3 && 2 * (2 * kASlot + 2 * ((c * bk * 2 + 1023) & ~1023)) + 2048 + kEpiStageBytes > g_max_smem) continue;   // needs >= 2 stages
+    if (x3 && 2 * (2 * kASlot + 2 * ((c * bk * 2 + 1023) & ~1023)) + 2048 + kEpiStageBytes > max_smem) continue;   // needs >= 2 stages
     const double t_kb = t_mma > t_fill ? t_mma : t_fill;
     int max_ks = 1;
-    if (allow_split && tiles * 2 <= g_num_sms && tiles * 2 <= kMaxCounterTiles) {
-      max_ks = int(g_num_sms / tiles);          // one wave of (tile, slice) items (a performance choice: nothing spins)
+    if (allow_split && tiles * 2 <= num_sms && tiles * 2 <= kMaxCounterTiles) {
+      max_ks = int(num_sms / tiles);            // one wave of (tile, slice) items (a performance choice: nothing spins)
       if (max_ks > num_kb / 2) max_ks = num_kb / 2;
       if (max_ks > 32) max_ks = 32;
       if (max_ks < 1) max_ks = 1;
@@ -926,7 +953,7 @@ static void pick_tiling(int N, int m_tiles, int num_kb, int bk, uint32_t a_bytes
       if (ks_eff != ks) continue;
       if (ks > 1 && size_t(tiles) * ks * 128 * c * 4 > kWsBytes) continue;
       const long items = tiles * ks;
-      const long waves = (items + g_num_sms - 1) / g_num_sms;
+      const long waves = (items + num_sms - 1) / num_sms;
       // split-K overhead: park one fp32 partial tile + read one tile's worth back (distributed reduce) at ~100 GB/s/SM
       double t_split = ks > 1 ? 2.0 + 2.0 * (128.0 * c * 4.0 / 100000.0) : 0.0;
       double t_kb_ = t_kb;
@@ -948,22 +975,48 @@ static void pick_tiling(int N, int m_tiles, int num_kb, int bk, uint32_t a_bytes
   *ksplit_out = best_ks;
 }
 
-int gemm_launch(const ConvGemm& d, cudaStream_t st) {
-  if (int e = device_setup()) return e;
-  GemmArgs g{};
-  CUtensorMap tmA, tmB;
+// What cuTensorMapEncodeTiled is asked to encode: dims (elements), strides of dims 1.. (bytes), box (elements).
+struct TmaGeom {
+  int rank;
+  cuuint64_t dims[5], strides[4];
+  cuuint32_t box[5];
+  CUtensorMapSwizzle swizzle;   // must span exactly one box row (bk * 2 bytes) and match the wgmma descriptors' layout
+};
+static int swizzle_bytes(CUtensorMapSwizzle s) {
+  return s == CU_TENSOR_MAP_SWIZZLE_128B ? 128 : s == CU_TENSOR_MAP_SWIZZLE_64B ? 64 : s == CU_TENSOR_MAP_SWIZZLE_32B ? 32 : 0;
+}
+static int desc_swizzle_bytes(uint64_t desc_hi) {   // layout field [62,64) of the smem matrix descriptor
+  const int layout = int(desc_hi >> 62);
+  return layout == 1 ? 128 : layout == 2 ? 64 : layout == 3 ? 32 : 0;
+}
+// One launch, fully planned on the host: the kernel arguments (minus the split-K workspace, counters and trace buffer,
+// which belong to the launching stream), both tensor maps' geometry, the grid and the dynamic shared memory.
+struct GemmPlan {
+  GemmArgs g;
+  TmaGeom ta, tb;
+  int kb_merge, grid;
+  size_t smem;
+};
+
+// Plans one launch for a device with num_sms SMs and max_smem bytes of opt-in shared memory per block; makes every
+// host-side rejection of gemm_launch and touches no device state.  have_ws: a split-K workspace slot is available for the
+// launching stream (otherwise K is never split and park-only launches are refused).
+static int plan_gemm(const ConvGemm& d, int num_sms, int max_smem, const GemmKnobs& kn, bool have_ws, GemmPlan* p) {
+  *p = GemmPlan{};
+  GemmArgs& g = p->g;
+  TmaGeom& ta = p->ta;
+  TmaGeom& tb = p->tb;
   const int Ktot = (d.mode == 0) ? d.K : 9 * d.Cin;
   const int kred = (d.mode == 0) ? d.K : d.Cin;
   // fp16x3 operands always stream 32-wide k-blocks (GemmArgs::x3).  The tiling and split-K choice is still made for 64-wide
   // blocks where K allows them (kb_merge = 2), so split-K slices start at the same K offsets and every sum keeps its order.
   const int bk = (kred % 64 == 0 && !d.x3) ? 64 : 32;
   const int kb_merge = (d.x3 && kred % 64 == 0) ? 2 : 1;
+  p->kb_merge = kb_merge;
   if (d.mode != 0 && kred % 32 != 0) return set_error("conv3x3: Cin must be a multiple of 32");
   if (d.mode == 0 && (d.K % 8 != 0 || d.lda % 8 != 0)) return set_error("gemm: K and lda must be multiples of 8");
   if ((reinterpret_cast<uintptr_t>(d.A) & 15) || (reinterpret_cast<uintptr_t>(d.B) & 15)) return set_error("gemm: operands must be 16-byte aligned");
-  static const bool no_halo = getenv("B2P_NO_HALO") != nullptr;
-  static const bool no_halo32 = getenv("B2P_NO_HALO32") != nullptr;
-  const bool halo = (d.mode == 1) && !no_halo && (bk == 64 || !no_halo32) && !d.x3;
+  const bool halo = (d.mode == 1) && !kn.no_halo && (bk == 64 || !kn.no_halo32) && !d.x3;
   if (d.x3 && (kred % bk != 0)) return set_error("gemm: fp16x3 operands need K (Cin) to be a multiple of 32");
   if (d.x3 && d.bf16) return set_error("gemm: fp16x3 operands are fp16");
   const int xk = d.x3 ? 2 : 1;   // operand rows carry [hi | lo]
@@ -992,11 +1045,8 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
     g.num_kb = (d.K + bk - 1) / bk;
     g.m_tiles = (d.M + kTileM - 1) / kTileM;
     g.a_bytes = kTileM * bk * 2;
-    cuuint64_t dims[2] = {cuuint64_t(a_span), cuuint64_t(d.M)};
-    cuuint64_t str[1] = {cuuint64_t(d.lda) * 2};
-    cuuint32_t box[2] = {cuuint32_t(bk), cuuint32_t(kTileM)};
     if (d.x3 && d.lda < a_span) return set_error("gemm: fp16x3 A rows are [hi(K) .. | lo(K) ..]: lda must be >= lo offset + K");
-    if (int e = encode(&tmA, d.bf16, 2, d.A, dims, str, box, bk)) return e;
+    ta = TmaGeom{2, {cuuint64_t(a_span), cuuint64_t(d.M)}, {cuuint64_t(d.lda) * 2}, {cuuint32_t(bk), cuuint32_t(kTileM)}};
   } else {
     const int s = (d.mode == 2) ? 2 : 1;
     if (s == 2 && ((d.H & 1) || (d.W & 1))) return set_error("conv3x3 s2: H and W must be even");
@@ -1044,43 +1094,34 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
     g.m_tiles = (g.nb > 1) ? (d.batch + g.nb - 1) / g.nb : g.tiles_x * g.tiles_y * d.batch;
     const cuuint64_t ld = cuuint64_t(d.lda);
     if (halo) {
-      cuuint64_t dims[4] = {cuuint64_t(d.Cin), cuuint64_t(d.W), cuuint64_t(d.H), cuuint64_t(d.batch)};
-      cuuint64_t str[3] = {ld * 2, ld * 2 * d.W, ld * 2 * d.W * d.H};
-      cuuint32_t box[4] = {cuuint32_t(bk), cuuint32_t(btw + 2), cuuint32_t(bth + 2), 1};
-      if (int e = encode(&tmA, d.bf16, 4, d.A, dims, str, box, bk)) return e;
+      ta = TmaGeom{4, {cuuint64_t(d.Cin), cuuint64_t(d.W), cuuint64_t(d.H), cuuint64_t(d.batch)}, {ld * 2, ld * 2 * d.W, ld * 2 * d.W * d.H},
+                   {cuuint32_t(bk), cuuint32_t(btw + 2), cuuint32_t(bth + 2), 1}};
     } else if (d.mode == 1) {
-      cuuint64_t dims[4] = {cuuint64_t(a_span), cuuint64_t(d.W), cuuint64_t(d.H), cuuint64_t(d.batch)};
-      cuuint64_t str[3] = {ld * 2, ld * 2 * d.W, ld * 2 * d.W * d.H};
-      cuuint32_t box[4] = {cuuint32_t(bk), cuuint32_t(btw), cuuint32_t(bth), cuuint32_t(g.nb)};
-      if (int e = encode(&tmA, d.bf16, 4, d.A, dims, str, box, bk)) return e;
+      ta = TmaGeom{4, {cuuint64_t(a_span), cuuint64_t(d.W), cuuint64_t(d.H), cuuint64_t(d.batch)}, {ld * 2, ld * 2 * d.W, ld * 2 * d.W * d.H},
+                   {cuuint32_t(bk), cuuint32_t(btw), cuuint32_t(bth), cuuint32_t(g.nb)}};
     } else {
       // (x parity, channel) merged in dim0: element (n, 2*yo+py, 2*xo+px, c) at c + px*ld  (+ xo*2ld + py*W*ld + yo*2W*ld)
       g.ldpar = int(d.lda);   // producer adds px * ldA to the channel coordinate
-      cuuint64_t dims[5] = {ld + cuuint64_t(a_span), cuuint64_t(d.W / 2), 2, cuuint64_t(d.H / 2), cuuint64_t(d.batch)};
-      cuuint64_t str[4] = {ld * 4, ld * 2 * d.W, ld * 4 * d.W, ld * 2 * d.W * d.H};
-      cuuint32_t box[5] = {cuuint32_t(bk), cuuint32_t(btw), 1, cuuint32_t(bth), cuuint32_t(g.nb)};
-      if (int e = encode(&tmA, d.bf16, 5, d.A, dims, str, box, bk)) return e;
+      ta = TmaGeom{5, {ld + cuuint64_t(a_span), cuuint64_t(d.W / 2), 2, cuuint64_t(d.H / 2), cuuint64_t(d.batch)},
+                   {ld * 4, ld * 2 * d.W, ld * 4 * d.W, ld * 2 * d.W * d.H}, {cuuint32_t(bk), cuuint32_t(btw), 1, cuuint32_t(bth), cuuint32_t(g.nb)}};
     }
   }
   int bn = 16, ksplit = 1;
-  static const bool no_split = getenv("B2P_NO_SPLITK") != nullptr;
-  const int slot = (no_split || d.no_split) ? -1 : ws_slot_for(st);
   pick_tiling(d.N, g.m_tiles, g.num_kb / kb_merge, (halo ? 9 * bk : bk) * kb_merge, g.a_bytes * kb_merge, d.bn_max > 0 ? d.bn_max : 256,
-              slot >= 0, d.x3 != 0, &bn, &ksplit);
+              have_ws, d.x3 != 0, num_sms, max_smem, kn, &bn, &ksplit);
   // Resident weights: one N tile, no split-K, at least one full wave of M tiles, and the whole weight matrix + a >= 2-deep
   // A ring must fit in shared memory (see GemmArgs::bres).
-  static const bool no_res = getenv("B2P_NO_BRES") != nullptr;
   bool bres = false;
   int res_slots = 0, res_stagesA = 0;
   const uint32_t a_slot_sep = halo ? g.a_slot : uint32_t(kASlot);
-  if (!no_res && !d.x3 && d.N <= 256 && g.m_tiles >= g_num_sms && (d.bn_max <= 0 || d.bn_max >= d.N)) {
+  if (!kn.no_bres && !d.x3 && d.N <= 256 && g.m_tiles >= num_sms && (d.bn_max <= 0 || d.bn_max >= d.N)) {
     static const int cand[] = {16, 32, 48, 64, 96, 128, 192, 256};
     int bnr = 256;
     for (int c : cand) if (c >= d.N) { bnr = c; break; }
     const uint32_t bslot = (uint32_t(bnr) * bk * 2 + 1023) & ~1023u;
     res_slots = halo ? g.cin_blocks * 9 : g.num_kb;
     const long long bar_bytes = 8LL * (2 * res_slots + 4 + 2 * 8) + 64;
-    const long long avail = (long long)g_max_smem - 1024 - kEpiStageBytes - ((bar_bytes + 1023) & ~1023LL) - (long long)res_slots * bslot;
+    const long long avail = (long long)max_smem - 1024 - kEpiStageBytes - ((bar_bytes + 1023) & ~1023LL) - (long long)res_slots * bslot;
     if (avail >= 2LL * a_slot_sep) {
       bres = true;
       bn = bnr;
@@ -1090,7 +1131,7 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
     }
   }
   if (d.park) {
-    if (d.mode != 0 || slot < 0) return set_error("gemm (park-only): needs mode 0 and a split-K workspace slot for this stream");
+    if (d.mode != 0 || !have_ws) return set_error("gemm (park-only): needs mode 0 and a split-K workspace slot for this stream");
     if (size_t(g.m_tiles) * ((d.N + bn - 1) / bn) * ksplit * 128 * bn * 4 > kWsBytes) return set_error("gemm (park-only): partial tiles exceed the workspace");
     bres = false;
   }
@@ -1099,24 +1140,17 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   g.sep = (halo || bres) ? 1 : 0;
   g.taps = halo ? 9 : 1;
   g.bn = bn;
-  static const bool sk_last = getenv("B2P_SPLITK_LAST") != nullptr;
-  g.sk_last = sk_last ? 1 : 0;
+  g.sk_last = kn.sk_last ? 1 : 0;
   g.ksplit = ksplit;
   g.kb_per = kb_merge * ((g.num_kb / kb_merge + ksplit - 1) / ksplit);
-  g.ws = slot >= 0 ? g_ws[slot] : nullptr;
-  g.counters = slot >= 0 ? g_counters[slot] : nullptr;
   g.n_tiles = (d.N + bn - 1) / bn;
   // co-scheduled CTAs should share the LARGER operand through L2: weights bigger than activations -> M tiles fastest
   g.mt_fast = (d.mode == 0 && g.m_tiles > 1 && (long long)d.N > (long long)d.M) ? 1 : 0;
   g.b_bytes = uint32_t(bn) * bk * 2;
   g.b_slot = (g.b_bytes + 1023) & ~1023u;
   g.bf16 = d.bf16 ? 1 : 0;
-  {
-    cuuint64_t dims[2] = {cuuint64_t(xk) * cuuint64_t(Ktot), cuuint64_t(d.N)};
-    cuuint64_t str[1] = {cuuint64_t(xk) * cuuint64_t(Ktot) * 2};
-    cuuint32_t box[2] = {cuuint32_t(bk), cuuint32_t(bn)};
-    if (int e = encode(&tmB, d.bf16, 2, d.B, dims, str, box, bk)) return e;
-  }
+  tb = TmaGeom{2, {cuuint64_t(xk) * cuuint64_t(Ktot), cuuint64_t(d.N)}, {cuuint64_t(xk) * cuuint64_t(Ktot) * 2}, {cuuint32_t(bk), cuuint32_t(bn)}};
+  ta.swizzle = tb.swizzle = (bk == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   g.d_ksplit = FastDiv::make(g.ksplit); g.d_ntiles = FastDiv::make(g.n_tiles); g.d_mtiles = FastDiv::make(g.m_tiles);
   g.d_perimg = FastDiv::make(d.mode != 0 ? g.tiles_x * g.tiles_y : 1); g.d_tilesx = FastDiv::make(d.mode != 0 ? g.tiles_x : 1);
   g.d_cinb = FastDiv::make(d.mode != 0 ? g.cin_blocks : 1);
@@ -1130,42 +1164,69 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
     bar_space = int((8LL * (2 * stages + 4 + 2 * g.stagesA) + 64 + 1023) & ~1023LL);
   } else if (halo) {
     // B ring first (up to 8 taps in flight), then as deep an A ring as fits (2..4 halo tiles)
-    stages = (g_max_smem - 1024 - 512 - kEpiStageBytes - 2 * int(g.a_slot)) / stage_bytes;
+    stages = (max_smem - 1024 - 512 - kEpiStageBytes - 2 * int(g.a_slot)) / stage_bytes;
     if (stages > kMaxStages) stages = kMaxStages;
     if (stages < 2) stages = 2;
-    int sa = (g_max_smem - 1024 - 512 - kEpiStageBytes - stages * stage_bytes) / int(g.a_slot);
+    int sa = (max_smem - 1024 - 512 - kEpiStageBytes - stages * stage_bytes) / int(g.a_slot);
     g.stagesA = sa > 4 ? 4 : (sa < 2 ? 2 : sa);
   } else {
     g.stagesA = 0;
-    stages = (g_max_smem - 1024 - 512 - kEpiStageBytes) / stage_bytes;
+    stages = (max_smem - 1024 - 512 - kEpiStageBytes) / stage_bytes;
     if (stages > kMaxStages) stages = kMaxStages;
     if (stages > g.kb_per && g.kb_per >= 2 && g.ksplit == 1) stages = g.kb_per;
     if (stages < 2) stages = 2;
   }
   const int a_region = g.sep ? g.stagesA * int(g.a_slot) : 0;
   g.stages = stages;
-  const size_t smem = size_t(a_region) + size_t(stages) * stage_bytes + 1024 + kEpiStageBytes + bar_space;
-  if (smem > size_t(g_max_smem)) return set_error("gemm: internal error, shared-memory plan exceeds the device limit");
+  p->smem = size_t(a_region) + size_t(stages) * stage_bytes + 1024 + kEpiStageBytes + bar_space;
+  if (p->smem > size_t(max_smem)) return set_error("gemm: internal error, shared-memory plan exceeds the device limit");
   // vector epilogue needs 16-byte aligned rows in out / residual and bias
   const int esz = d.out_f32 ? 4 : 2;
   g.vec_ok = ((reinterpret_cast<uintptr_t>(d.out) & 15) == 0) && ((d.ldc * esz) % 16 == 0) &&
              (!d.res || (((reinterpret_cast<uintptr_t>(d.res) & 15) == 0) && ((d.ldr * esz) % 16 == 0))) &&
              (!d.bias || ((reinterpret_cast<uintptr_t>(d.bias) & 15) == 0));
+  const int total = g.m_tiles * g.n_tiles * g.ksplit;
+  int grid = total < num_sms ? total : num_sms;
+  if (kn.max_grid > 0 && grid > kn.max_grid && ksplit == 1) grid = kn.max_grid;
+  p->grid = grid;
+  return 0;
+}
+
+static int encode(CUtensorMap* m, int bf16, const TmaGeom& t, const void* base) {
+  return encode(m, bf16, t.rank, base, t.dims, t.strides, t.box, t.swizzle);
+}
+
+static void plan_fields(const GemmPlan& p, int* out);
+// the plan of the calling thread's most recent launch (b2p_gemm_last_plan): the one actually launched, after the stream's
+// split-K workspace slot was looked up
+static thread_local int t_last_plan[kGemmPlanFields];
+static thread_local bool t_have_last_plan = false;
+
+int gemm_launch(const ConvGemm& d, cudaStream_t st) {
+  if (int e = device_setup()) return e;
+  const GemmKnobs& kn = gemm_knobs();
+  const int slot = (kn.no_split || d.no_split) ? -1 : ws_slot_for(st);
+  GemmPlan p;
+  if (int e = plan_gemm(d, g_num_sms, g_max_smem, kn, slot >= 0, &p)) return e;
+  GemmArgs& g = p.g;
+  g.ws = slot >= 0 ? g_ws[slot] : nullptr;
+  g.counters = slot >= 0 ? g_counters[slot] : nullptr;
+  CUtensorMap tmA, tmB;
+  if (int e = encode(&tmA, d.bf16, p.ta, d.A)) return e;
+  if (int e = encode(&tmB, d.bf16, p.tb, d.B)) return e;
+  const int grid = p.grid, bn = g.bn, ksplit = g.ksplit;
+  const int Ktot = (d.mode == 0) ? d.K : 9 * d.Cin;
   static const bool dbg = getenv("B2P_DEBUG") != nullptr;
   static const bool no_pdl = getenv("B2P_NO_PDL") != nullptr;
-  const int total = g.m_tiles * g.n_tiles * g.ksplit;
-  static const int max_grid = getenv("B2P_MAX_GRID") ? atoi(getenv("B2P_MAX_GRID")) : 0;   // experiment: leave SMs to other streams
-  int grid = total < g_num_sms ? total : g_num_sms;
-  if (max_grid > 0 && grid > max_grid && ksplit == 1) grid = max_grid;
   if (grid <= 0) return 0;
   if (dbg)
     fprintf(stderr, "b2p_gemm mode=%d M=%d N=%d Ktot=%d bk=%d bn=%d tw=%d th=%d m_tiles=%d n_tiles=%d stages=%d grid=%d act=%d f32=%d res=%d ksplit=%d x3=%d bres=%d stagesA=%d\n",
-            g.mode, d.mode == 0 ? d.M : g.m_tiles * 128, d.N, Ktot, bk, bn, g.tw, g.th, g.m_tiles, g.n_tiles, stages, grid,
+            g.mode, d.mode == 0 ? d.M : g.m_tiles * 128, d.N, Ktot, g.bk, bn, g.tw, g.th, g.m_tiles, g.n_tiles, g.stages, grid,
             d.act, d.out_f32, d.res != nullptr, ksplit, g.x3, g.bres, g.stagesA);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
+  cfg.dynamicSmemBytes = p.smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -1188,10 +1249,49 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   if (ce == cudaSuccess) ce = cudaGetLastError();
   if (ce != cudaSuccess) return set_error(cudaGetErrorString(ce));
   count_launch();
+  plan_fields(p, t_last_plan);
+  t_have_last_plan = true;
   if (d.park_info) {
     d.park_info->ws = g.ws; d.park_info->bn = bn; d.park_info->ksplit = g.ksplit; d.park_info->n_tiles = g.n_tiles;
     d.park_info->m_tiles = g.m_tiles; d.park_info->mt_fast = g.mt_fast;
   }
+  return 0;
+}
+
+// Elements from a tensor map's base pointer up to one past the last element it can address.
+static long long tma_extent(const TmaGeom& t) {
+  long long e = (long long)t.dims[0];
+  for (int i = 1; i < t.rank; ++i) e += (long long)(t.dims[i] - 1) * (long long)(t.strides[i - 1] / 2);
+  return e;
+}
+
+static void plan_fields(const GemmPlan& p, int* out) {
+  const GemmArgs& g = p.g;
+  auto sat = [](long long v) { return int(v > 0x7fffffffLL ? 0x7fffffffLL : v); };
+  const int f[] = {g.mode, g.bk, g.bn, g.ksplit, g.kb_per, p.kb_merge, g.stages, g.stagesA, g.sep, g.bres, g.nb, g.tw, g.tw_valid,
+                   g.th, g.m_tiles, g.n_tiles, g.mt_fast, p.grid, int(p.smem), g.vec_ok, g.split, g.res_lo, g.park,
+                   g.x3, g.num_kb, g.taps, int(g.a_bytes), int(g.a_slot), int(g.b_bytes), int(g.b_slot), g.tiles_x, g.tiles_y,
+                   p.ta.rank, int(p.ta.box[0]), int(p.ta.box[1]), int(p.ta.box[2]), int(p.ta.box[3]), int(p.ta.box[4]),
+                   int(p.tb.box[0]), int(p.tb.box[1]), sat(tma_extent(p.ta)), sat(tma_extent(p.tb)),
+                   swizzle_bytes(p.ta.swizzle), swizzle_bytes(p.tb.swizzle), desc_swizzle_bytes(g.desc_hi)};
+  static_assert(sizeof(f) / sizeof(f[0]) == kGemmPlanFields, "b2p_gemm_plan field count");
+  for (int i = 0; i < kGemmPlanFields; ++i) out[i] = f[i];
+}
+
+// Host-only planner (b2p_gemm_plan): see include/b200parse.h for the field order of `out`.  The plan assumes the launching
+// stream owns a split-K workspace slot (gemm_launch plans without split-K once kWsSlots streams own one).
+int gemm_plan_host(const ConvGemm& d, int num_sms, int max_smem, int* out) {
+  if (num_sms < 1 || max_smem < 1) return set_error("gemm_plan: num_sms and max_smem must be positive");
+  const GemmKnobs& kn = gemm_knobs();
+  GemmPlan p;
+  if (int e = plan_gemm(d, num_sms, max_smem, kn, !(kn.no_split || d.no_split), &p)) return e;
+  plan_fields(p, out);
+  return 0;
+}
+
+int gemm_last_plan(int* out) {
+  if (!t_have_last_plan) return set_error("gemm_last_plan: this thread has launched no GEMM/conv");
+  for (int i = 0; i < kGemmPlanFields; ++i) out[i] = t_last_plan[i];
   return 0;
 }
 
