@@ -78,6 +78,16 @@ int b2p_gemm_plan(const void* in, long long ld_in, int batch, int H, int W, int 
                   long long lo_a, long long lo_out, long long lo_res, int num_sms, int max_smem, int* plan_host);
 /* Host only: the same 45 fields for the most recent GEMM/conv launch made by the calling thread (-1 if it made none). */
 int b2p_gemm_last_plan(int* plan_host);
+/* Host only: the epilogue of the plan b2p_gemm_plan makes for the same arguments.  epi_host receives 24 ints:
+ *   0 TMA epilogue (1) or register epilogue (0), 1 columns per chunk, 2 chunks per tile, 3 staging buffers,
+ *   4 output planes (2 = fp16 [hi | lo] pair), 5 residual buffers, 6 residual planes (0 = no residual),
+ *   7 shared memory of the epilogue (bytes), 8 stages, 9 stagesA, 10 smem (as b2p_gemm_plan fields 6, 7, 18),
+ *   11 rank of the output tensor map, 12-14 its box (elements, unused dims 0), 15-16 its global strides of dims 1, 2 (bytes),
+ *   17-22 the same for the residual tensor map (rank 0 = none), 23 swizzle span (bytes) of both.
+ * Fields 11-23 are 0 for the register epilogue. */
+int b2p_gemm_epilogue_plan(const void* in, long long ld_in, int batch, int H, int W, int Cin, int stride, const void* weight, int Cout,
+                           void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act, int flags,
+                           long long lo_a, long long lo_out, long long lo_res, int num_sms, int max_smem, int* epi_host);
 
 /* ---- YOLOv9-E graph helpers (inside the TorchScript archive, ref:util/yolov9.py:120-121) ----
  * `_x3` forms: every map is an fp16 hi/lo pair (lo plane `lo*` elements after the hi plane, 0 = plain fp16); the

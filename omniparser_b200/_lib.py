@@ -30,6 +30,7 @@ PROTOTYPES = {
     "b2p_conv3x3_planes": (i32, [vp, i64, i32, i32, i32, i32, i32, vp, i32, vp, i64, vp, vp, i64, i32, i32, i64, i64, i64, vp]),
     "b2p_gemm_plan": (i32, [vp, i64, i32, i32, i32, i32, i32, vp, i32, vp, i64, vp, vp, i64, i32, i32, i64, i64, i64, i32, i32, vp]),
     "b2p_gemm_last_plan": (i32, [vp]),
+    "b2p_gemm_epilogue_plan": (i32, [vp, i64, i32, i32, i32, i32, i32, vp, i32, vp, i64, vp, vp, i64, i32, i32, i64, i64, i64, i32, i32, vp]),
     "b2p_adown_pool": (i32, [vp, i64, i32, i32, i32, i32, vp, i64, vp, i64, vp]),
     "b2p_adown_pool_x3": (i32, [vp, i64, i32, i32, i32, i32, vp, i64, vp, i64, i64, i64, i64, vp]),
     "b2p_maxpool_s1_x3": (i32, [vp, i64, i32, i32, i32, i32, i32, vp, i64, i64, i64, vp]),

@@ -98,10 +98,9 @@ int b2p_conv3x3(const void* in, long long ld_in, int batch, int H, int W, int Ci
 // Host only: the launch plan b2p_conv3x3_planes (stride 1 | 2) or b2p_gemm_planes (stride 0: M = batch, K = Cin; H, W
 // ignored) would make on a device with num_sms SMs and max_smem bytes of opt-in shared memory per block.  flags bit 5:
 // plan the park-only GEMM of b2p_gemm_ln.  No device is touched.
-int b2p_gemm_plan(const void* in, long long ld_in, int batch, int H, int W, int Cin, int stride, const void* weight, int Cout,
-                  void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act, int flags,
-                  long long lo_a, long long lo_out, long long lo_res, int num_sms, int max_smem, int* plan_host) {
-  if (stride != 0 && stride != 1 && stride != 2) return set_error("gemm_plan: stride must be 0 (GEMM), 1 or 2");
+static ConvGemm plan_call(const void* in, long long ld_in, int batch, int H, int W, int Cin, int stride, const void* weight,
+                          int Cout, void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act,
+                          int flags, long long lo_a, long long lo_out, long long lo_res) {
   ConvGemm d{};
   d.mode = stride; d.bf16 = flags & 1; d.A = in; d.lda = ld_in; d.B = weight; d.N = Cout;
   if (stride == 0) { d.M = batch; d.K = Cin; }
@@ -110,7 +109,22 @@ int b2p_gemm_plan(const void* in, long long ld_in, int batch, int H, int W, int 
   d.bn_max = (flags >> 8) & 0x1ff; d.no_split = (flags >> 4) & 1; d.split_out = (flags >> 2) & 1; d.x3 = (flags >> 3) & 1;
   d.lo_a = lo_a; d.lo_out = lo_out; d.lo_res = lo_res;
   d.park = (flags >> 5) & 1;
-  return gemm_plan_host(d, num_sms, max_smem, plan_host);
+  return d;
+}
+int b2p_gemm_plan(const void* in, long long ld_in, int batch, int H, int W, int Cin, int stride, const void* weight, int Cout,
+                  void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act, int flags,
+                  long long lo_a, long long lo_out, long long lo_res, int num_sms, int max_smem, int* plan_host) {
+  if (stride != 0 && stride != 1 && stride != 2) return set_error("gemm_plan: stride must be 0 (GEMM), 1 or 2");
+  return gemm_plan_host(plan_call(in, ld_in, batch, H, W, Cin, stride, weight, Cout, out, ldc, bias, residual, ldr, act, flags, lo_a,
+                                  lo_out, lo_res), num_sms, max_smem, plan_host);
+}
+// Host only: the epilogue part of the same plan (see include/b200parse.h).
+int b2p_gemm_epilogue_plan(const void* in, long long ld_in, int batch, int H, int W, int Cin, int stride, const void* weight, int Cout,
+                           void* out, long long ldc, const float* bias, const void* residual, long long ldr, int act, int flags,
+                           long long lo_a, long long lo_out, long long lo_res, int num_sms, int max_smem, int* epi_host) {
+  if (stride != 0 && stride != 1 && stride != 2) return set_error("gemm_plan: stride must be 0 (GEMM), 1 or 2");
+  return gemm_epilogue_plan_host(plan_call(in, ld_in, batch, H, W, Cin, stride, weight, Cout, out, ldc, bias, residual, ldr, act, flags,
+                                           lo_a, lo_out, lo_res), num_sms, max_smem, epi_host);
 }
 // Host only: the plan fields of the calling thread's most recent GEMM/conv launch (what was launched, as b2p_gemm_plan).
 int b2p_gemm_last_plan(int* plan_host) { return gemm_last_plan(plan_host); }

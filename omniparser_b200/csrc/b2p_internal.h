@@ -58,7 +58,10 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st);
 // only: kGemmPlanFields ints in the order of b2p_gemm_plan (include/b200parse.h).
 static constexpr int kGemmPlanFields = 45;
 int gemm_plan_host(const ConvGemm& d, int num_sms, int max_smem, int* out);
-int gemm_last_plan(int* out);   // the same fields for the calling thread's most recent launch
+int gemm_last_plan(int* out);
+// host only: kEpiPlanFields ints in the order of b2p_gemm_epilogue_plan (include/b200parse.h)
+static constexpr int kEpiPlanFields = 24;
+int gemm_epilogue_plan_host(const ConvGemm& d, int num_sms, int max_smem, int* out);   // the same fields for the calling thread's most recent launch
 int trace_read(unsigned long long* stamps, int* meta, int max_launches);   // B2P_TRACE=1 debugging aid
 
 // Second-version SIMT kernels of the caption encoder (florence_simt.cu).  Return 0 = launched, 1 = shape not covered (the caller

@@ -93,6 +93,12 @@ struct GemmArgs {
   int park;        // 1 = park-only: every (tile, k slice) leaves its raw fp32 accumulators in ws and the kernel ends; the
                    // following kernel (splitk_ln_kernel) sums the slices, adds bias + residual and applies LayerNorm
   unsigned long long* trace;   // B2P_TRACE=1 only, else null: [CTA][16] globaltimer stamps (see trace_stamp)
+  // TMA epilogue (mode 0, direct launches only, see plan_epilogue): each 64-byte-wide column chunk of the whole 128-row
+  // tile is built in one of two shared-memory staging buffers and written by one TMA store (tmC); the residual of the
+  // chunk arrives by TMA (tmR) into one of two residual buffers, issued two chunks ahead (the first two at item start, so
+  // they land under the tile's MMAs).  epi_bytes = the epilogue's shared-memory region either way.
+  int tma_epi, out_planes, res_planes;   // planes: 2 = a [hi | lo] fp16 pair (split output / res_lo), 1 = one plane
+  uint32_t epi_buf, res_buf, epi_bytes;  // bytes of one staging / residual buffer, of the whole region
 };
 
 // Shared-memory matrix descriptor (PTX ISA "wgmma matrix descriptor"), K-major operand, swizzled:
@@ -135,17 +141,18 @@ __device__ __forceinline__ float act_fn(float x, int act) {
   if (act == 2) return gelu_fn(x);
   return x;
 }
-// Activation of 16 accumulator columns.  The switch on the (runtime) activation code sits OUTSIDE the element loop: with
+// Activation of N accumulator columns.  The switch on the (runtime) activation code sits OUTSIDE the element loop: with
 // act_fn(x[j], act) inside it the compiler kept one basic block per element (uniform branch, then the dependent
 // FMUL -> MUFU.EX2 -> FADD -> MUFU.RCP -> FMUL chain), so the 16 chains run back to back at full MUFU latency instead of
 // interleaved.
-__device__ __forceinline__ void act16(float (&x)[16], int act) {
+template <int N>
+__device__ __forceinline__ void act_n(float (&x)[N], int act) {
   if (act == 1) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) x[j] = silu_fn(x[j]);
+    for (int j = 0; j < N; ++j) x[j] = silu_fn(x[j]);
   } else if (act == 2) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) x[j] = gelu_fn(x[j]);
+    for (int j = 0; j < N; ++j) x[j] = gelu_fn(x[j]);
   }
 }
 
@@ -167,7 +174,7 @@ __device__ __forceinline__ void epi_store16(const GemmArgs& g, const EpiCtx& e, 
         x[4 * q + 0] += b.x; x[4 * q + 1] += b.y; x[4 * q + 2] += b.z; x[4 * q + 3] += b.w;
       }
     }
-    act16(x, g.act);
+    act_n(x, g.act);
     if (!valid) return;
     if (g.res) {
       if (g.out_f32) {
@@ -259,12 +266,144 @@ __device__ __forceinline__ void epi_store16(const GemmArgs& g, const EpiCtx& e, 
 }
 
 // Phase stamps of a traced launch (B2P_TRACE=1, tools/trace_gemm.py): where a launch's microseconds go.
-enum { kTrEntry = 0, kTrPrologue, kTrDepWait, kTrFirstTma, kTrFirstFull, kTrFirstAccDone, kTrFirstEpiStart, kTrLastEpiEnd, kTrExit };
+// Slots past kTrExit are not stamps but sums over all of the CTA's items: kTrSumMain = item start -> accumulators ready
+// (main loop, TMA waits included), kTrSumEpi = accumulators ready -> item end (epilogue, split-K reduction included);
+// kTrMark = start of the current phase.  They live in the stamp buffer: a register held across the main loop makes the
+// BN = 256 instantiation spill.
+enum { kTrEntry = 0, kTrPrologue, kTrDepWait, kTrFirstTma, kTrFirstFull, kTrFirstAccDone, kTrFirstEpiStart, kTrLastEpiEnd, kTrExit,
+       kTrSumMain, kTrSumEpi, kTrMark };
+__device__ __forceinline__ unsigned long long trace_now() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ unsigned long long& trace_at(const GemmArgs& g, int slot) { return g.trace[blockIdx.x * 16 + slot]; }
 __device__ __forceinline__ void trace_stamp(const GemmArgs& g, int slot) {
+  if (g.trace) trace_at(g, slot) = trace_now();
+}
+// adds the time since the last mark to the sum `slot` and marks now (call from one thread)
+__device__ __forceinline__ void trace_phase(const GemmArgs& g, int slot) {
   if (g.trace) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    g.trace[blockIdx.x * 16 + slot] = t;
+    const unsigned long long t = trace_now();
+    trace_at(g, slot) += t - trace_at(g, kTrMark);
+    trace_at(g, kTrMark) = t;
+  }
+}
+
+// TMA epilogue (GemmArgs::tma_epi).  A buffer holds [plane][128 rows][64 B] in the TMA 64-byte swizzle: 16-byte unit u of
+// row r sits at unit u ^ ((r >> 1) & 3), which makes the fragment's shared-memory accesses below bank-conflict free.
+static constexpr uint32_t kEpiPlane = kTileM * 64;
+// bias pair load that stays in program order (asm volatile): hoisted out of the chunk loop, the __ldg loads of a whole
+// BN = 256 tile would hold 128 registers next to the 128 accumulators
+__device__ __forceinline__ float2 ldg_f2_in_order(const float* p) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ float2 lds_h2(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return __half22float2(*reinterpret_cast<const __half2*>(&v));
+}
+__device__ __forceinline__ void sts_f2(uint32_t a, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ void sts_h2(uint32_t a, __half2 h) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(*reinterpret_cast<const uint32_t*>(&h)) : "memory");
+}
+// residual of column chunk c of the tile (mt, n0) into residual buffer c & 1 (one thread)
+__device__ __forceinline__ void epi_res_load(const GemmArgs& g, const CUtensorMap* tmR, int c, int mt, int n0, uint32_t rsb, uint32_t bar_res) {
+  const int cols = g.out_f32 ? 16 : 32;
+  const uint32_t bar = bar_res + 8u * uint32_t(c & 1);
+  const uint32_t dst = rsb + uint32_t(c & 1) * g.res_buf;
+  mbar_expect_tx(bar, g.res_buf);
+  if (g.res_planes == 2) tma_load_3d(dst, tmR, bar, n0 + c * cols, mt * kTileM, 0);
+  else tma_load_2d(dst, tmR, bar, n0 + c * cols, mt * kTileM);
+}
+// The epilogue of one direct mode-0 tile straight from the wgmma fragment (lane l of consumer warp w holds rows 16w + l/4
+// and 16w + l/4 + 8, and of each 8-column group the columns 2(l%4), +1), one 64-byte column chunk at a time.  Per element
+// the fp32 order of epi_store16: acc + bias -> activation -> + residual hi -> + residual lo -> round (lo = x - hi).
+// Staging buffer (sbuf & 1) is rewritten only after the store issued from it two chunks earlier has read it.
+template <int BN, bool F32>
+__device__ __forceinline__ void epi_tma(const GemmArgs& g, const CUtensorMap* tmC, const CUtensorMap* tmR, const float (&acc)[BN / 2],
+                                        int mt, int n0, int row, int ctid, uint32_t stg, uint32_t bar_res, uint32_t& sbuf,
+                                        uint32_t& rphase) {
+  constexpr int kCols = F32 ? 16 : 32;     // columns of a 64-byte chunk
+  constexpr int kGroups = kCols / 8;       // 8-column fragment groups per chunk
+  if constexpr (BN % kCols == 0) {
+    const int q = threadIdx.x & 3;
+    // byte offsets of this thread's column pair of group 0 in rows `row` and `row + 8`; group jj is at offset ^ (jj << 4)
+    // (fp32: ^ (jj << 5)) since the swizzle XORs 16-byte unit indices
+    const uint32_t sw = ((uint32_t(row) >> 1) & 3u) << 4;
+    const uint32_t in_row = F32 ? ((uint32_t(q >> 1) << 4) ^ sw) | (uint32_t(q & 1) << 3) : sw | (uint32_t(q) << 2);
+    const uint32_t offA = uint32_t(row) * 64u + in_row, offB = offA + 8u * 64u;
+    const uint32_t rsb = stg + 2 * g.epi_buf;
+#pragma unroll
+    for (int c = 0; c < BN / kCols; ++c) {
+      float x[4 * kGroups];
+#pragma unroll
+      for (int jj = 0; jj < kGroups; ++jj) {
+        const int a = (c * kGroups + jj) * 4;
+        const int col = n0 + c * kCols + 8 * jj + 2 * q;
+        float2 b = make_float2(0.f, 0.f);
+        if (g.bias && col < g.N) b = ldg_f2_in_order(g.bias + col);
+        x[4 * jj] = acc[a] + b.x; x[4 * jj + 1] = acc[a + 1] + b.y;
+        x[4 * jj + 2] = acc[a + 2] + b.x; x[4 * jj + 3] = acc[a + 3] + b.y;
+      }
+      act_n(x, g.act);
+      constexpr uint32_t kStep = F32 ? 32u : 16u;
+      if (g.res) {
+        mbar_wait(bar_res + 8u * uint32_t(c & 1), (rphase >> (c & 1)) & 1u);
+        rphase ^= 1u << (c & 1);
+        const uint32_t rb = rsb + uint32_t(c & 1) * g.res_buf;
+#pragma unroll
+        for (int jj = 0; jj < kGroups; ++jj) {
+          const uint32_t oa = offA ^ (uint32_t(jj) * kStep), ob = offB ^ (uint32_t(jj) * kStep);
+          if constexpr (F32) {
+            const float2 ta = lds_f2(rb + oa), tb = lds_f2(rb + ob);
+            x[4 * jj] += ta.x; x[4 * jj + 1] += ta.y; x[4 * jj + 2] += tb.x; x[4 * jj + 3] += tb.y;
+          } else {
+            for (int pl = 0; pl < g.res_planes; ++pl) {
+              const float2 ta = lds_h2(rb + pl * kEpiPlane + oa), tb = lds_h2(rb + pl * kEpiPlane + ob);
+              x[4 * jj] += ta.x; x[4 * jj + 1] += ta.y; x[4 * jj + 2] += tb.x; x[4 * jj + 3] += tb.y;
+            }
+          }
+        }
+      }
+      const uint32_t sb = stg + (sbuf & 1u) * g.epi_buf;
+#pragma unroll
+      for (int jj = 0; jj < kGroups; ++jj) {
+        const uint32_t oa = offA ^ (uint32_t(jj) * kStep), ob = offB ^ (uint32_t(jj) * kStep);
+        if constexpr (F32) {
+          sts_f2(sb + oa, x[4 * jj], x[4 * jj + 1]);
+          sts_f2(sb + ob, x[4 * jj + 2], x[4 * jj + 3]);
+        } else {
+          const __half2 ha = __floats2half2_rn(x[4 * jj], x[4 * jj + 1]), hb = __floats2half2_rn(x[4 * jj + 2], x[4 * jj + 3]);
+          sts_h2(sb + oa, ha);
+          sts_h2(sb + ob, hb);
+          if (g.out_planes == 2) {
+            const float2 fa = __half22float2(ha), fb = __half22float2(hb);
+            sts_h2(sb + kEpiPlane + oa, __floats2half2_rn(x[4 * jj] - fa.x, x[4 * jj + 1] - fa.y));
+            sts_h2(sb + kEpiPlane + ob, __floats2half2_rn(x[4 * jj + 2] - fb.x, x[4 * jj + 3] - fb.y));
+          }
+        }
+      }
+      fence_proxy_async_smem();
+      if (ctid == 0) bulk_wait_read<0>();   // the other buffer's store has read it: it may be rewritten after the barrier
+      asm volatile("bar.sync 2, %0;" ::"n"(kConsumerThreads) : "memory");
+      if (ctid == 0) {
+        if (g.out_planes == 2) tma_store_3d(tmC, sb, n0 + c * kCols, mt * kTileM, 0);
+        else tma_store_2d(tmC, sb, n0 + c * kCols, mt * kTileM);
+        bulk_commit();
+        if (g.res && c + 2 < BN / kCols) epi_res_load(g, tmR, c + 2, mt, n0, rsb, bar_res);
+      }
+      ++sbuf;
+    }
   }
 }
 
@@ -291,21 +430,26 @@ __device__ __forceinline__ void mma_stage_x3(float (&acc)[BN / 2], uint32_t a_hi
   }
 }
 
-template <int BN>
+// kTma: the instantiation of the launches planned with the TMA epilogue (direct mode-0 tiles only).  It is a kernel of its
+// own: compiled next to the register epilogue and the split-K paths, the TMA epilogue makes ptxas spill at BN = 192 / 256
+// (a register cap of 168 at 384 threads, 128 of them accumulators).
+template <int BN, bool kTma>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs g) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
+                  const __grid_constant__ CUtensorMap tmR, const GemmArgs g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t a_part = g.x3 ? 2u * g.a_slot : g.a_slot;                          // single ring: [A_hi][A_lo] | [A]
   const uint32_t stage_bytes = g.sep ? g.b_slot : a_part + (g.x3 ? 2u : 1u) * g.b_slot;
   const uint32_t a_region = g.sep ? uint32_t(g.stagesA) * g.a_slot : 0u;   // separate pipelines: [A slots][B slots]
   float* epi_stage = reinterpret_cast<float*>(smem + a_region + size_t(g.stages) * stage_bytes);   // [8 warps][16 rows][kStagePitch]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi_stage) + kEpiStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi_stage) + g.epi_bytes);
   const uint32_t bar_full = smem_u32(bars);
   const uint32_t bar_empty = bar_full + 8 * g.stages;
   const uint32_t bar_afull = bar_empty + 8 * g.stages;     // separate pipelines only
   const uint32_t bar_aempty = bar_afull + 8 * g.stagesA;
   uint32_t* s_flag = reinterpret_cast<uint32_t*>(bars + 2 * g.stages + 2 * g.stagesA);
+  const uint32_t bar_res = smem_u32(bars + 2 * g.stages + 2 * g.stagesA + 1);   // TMA epilogue: residual buffer 0 / 1 full
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -320,6 +464,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (kTma) {
+      tma_prefetch_desc(&tmC);
+      if (g.res) tma_prefetch_desc(&tmR);
+    }
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < g.stages; ++s) {
@@ -329,6 +477,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int a = 0; a < g.stagesA; ++a) {
       mbar_init(bar_afull + 8 * a, 1);
       mbar_init(bar_aempty + 8 * a, kConsumerGroups);
+    }
+    if (kTma) {
+      mbar_init(bar_res, 1);
+      mbar_init(bar_res + 8, 1);
     }
     mbar_fence_init();
   }
@@ -512,9 +664,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
   const bool r_ok = (r_sub < e_nb) && (r_ty < e_th) && (r_tx < e_twv);
 
+  uint32_t epi_sbuf = 0, epi_rphase = 0;   // TMA epilogue: staging buffers used so far; residual buffers' mbarrier parities
   for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    if (ctid == 0) trace_stamp(g, kTrMark);
     const int tile = e_dks.div(item);
     const int ks = item - tile * ksplit;
+    if (kTma && g.res && ctid == 0) {
+      // the tile's first two residual chunks land under its MMAs
+      const int mt_ = e_mtfast ? tile - e_dmt.div(tile) * g.m_tiles : e_dnt.div(tile);
+      const int n0_ = (e_mtfast ? e_dmt.div(tile) : tile - mt_ * g.n_tiles) * e_bn;
+      const uint32_t rsb = smem_u32(epi_stage) + 2 * g.epi_buf;
+      epi_res_load(g, &tmR, 0, mt_, n0_, rsb, bar_res);
+      if (BN > (g.out_f32 ? 16 : 32)) epi_res_load(g, &tmR, 1, mt_, n0_, rsb, bar_res);
+    }
     const int kb0 = ks * kb_per, kb1 = min(num_kb, kb0 + kb_per);
     float acc[BN / 2];           // this thread's fragment of the 64 x BN accumulator (layout: ptx.cuh)
 #pragma unroll
@@ -588,12 +750,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     wgmma_fence_operand(acc);
     retire(0u, 0u);
     if (item == blockIdx.x && ctid == 0) { trace_stamp(g, kTrFirstAccDone); trace_stamp(g, kTrFirstEpiStart); }
+    if (ctid == 0) trace_phase(g, kTrSumMain);
 
     // -------------------------------------------------------------- epilogue of this item
     int nt, mt;
     if (e_mtfast) { nt = e_dmt.div(tile); mt = tile - nt * g.m_tiles; }
     else { mt = e_dnt.div(tile); nt = tile - mt * g.n_tiles; }
     const int n0 = nt * e_bn;
+    if constexpr (kTma) {
+      const int row = cw * 64 + (warp & 3) * 16 + (lane >> 2);
+      const uint32_t stg = smem_u32(epi_stage);
+      if (g.out_f32) epi_tma<BN, true>(g, &tmC, &tmR, acc, mt, n0, row, ctid, stg, bar_res, epi_sbuf, epi_rphase);
+      else epi_tma<BN, false>(g, &tmC, &tmR, acc, mt, n0, row, ctid, stg, bar_res, epi_sbuf, epi_rphase);
+      if (ctid == 0) trace_phase(g, kTrSumEpi);
+      continue;
+    }
     long long pix;
     bool valid;
     if (e_mode == 0) {
@@ -782,7 +953,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
+    if (ctid == 0) trace_phase(g, kTrSumEpi);
   }
+  if (kTma && ctid == 0) bulk_wait_all();   // the stores are performed before the grid completes (PDL dependents)
   if (ctid == 0) { trace_stamp(g, kTrLastEpiEnd); trace_stamp(g, kTrExit); }
 }
 
@@ -802,12 +975,12 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-static int encode(CUtensorMap* m, int bf16, int rank, const void* base, const cuuint64_t* dims,
+static int encode(CUtensorMap* m, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
                   const cuuint64_t* strides_bytes, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn fn = get_encode();
   if (!fn) return set_error("cuTensorMapEncodeTiled entry point unavailable");
   cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank,
+  CUresult r = fn(m, dtype, rank,
                   const_cast<void*>(base), dims, strides_bytes, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -850,11 +1023,15 @@ static int g_trace_meta[kTraceCap][8];
 static std::mutex g_trace_mu;
 
 // one instantiation per N tile: the accumulator fragment (BN / 2 registers per consumer thread) is sized at compile time
-typedef void (*GemmKernel)(const CUtensorMap, const CUtensorMap, const GemmArgs);
+typedef void (*GemmKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmArgs);
 static constexpr int kNumBn = 8;
 static const int kBnCand[kNumBn] = {256, 192, 128, 96, 64, 48, 32, 16};
-static const GemmKernel kGemmKernels[kNumBn] = {gemm_wgmma_kernel<256>, gemm_wgmma_kernel<192>, gemm_wgmma_kernel<128>, gemm_wgmma_kernel<96>,
-                                                gemm_wgmma_kernel<64>,  gemm_wgmma_kernel<48>,  gemm_wgmma_kernel<32>,  gemm_wgmma_kernel<16>};
+// [N tile][TMA epilogue]
+static const GemmKernel kGemmKernels[kNumBn][2] = {
+    {gemm_wgmma_kernel<256, false>, gemm_wgmma_kernel<256, true>}, {gemm_wgmma_kernel<192, false>, gemm_wgmma_kernel<192, true>},
+    {gemm_wgmma_kernel<128, false>, gemm_wgmma_kernel<128, true>}, {gemm_wgmma_kernel<96, false>, gemm_wgmma_kernel<96, true>},
+    {gemm_wgmma_kernel<64, false>, gemm_wgmma_kernel<64, true>},   {gemm_wgmma_kernel<48, false>, gemm_wgmma_kernel<48, true>},
+    {gemm_wgmma_kernel<32, false>, gemm_wgmma_kernel<32, true>},   {gemm_wgmma_kernel<16, false>, gemm_wgmma_kernel<16, true>}};
 
 static std::mutex g_setup_mu;
 static int device_setup() {
@@ -869,8 +1046,9 @@ static int device_setup() {
   g_num_sms = p.multiProcessorCount;
   g_max_smem = int(p.sharedMemPerBlockOptin);
   for (int i = 0; i < kNumBn; ++i)
-    if (cudaFuncSetAttribute(kGemmKernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem) != cudaSuccess)
-      return set_error("cudaFuncSetAttribute(max dynamic smem) failed");
+    for (int t = 0; t < 2; ++t)
+      if (cudaFuncSetAttribute(kGemmKernels[i][t], cudaFuncAttributeMaxDynamicSharedMemorySize, g_max_smem) != cudaSuccess)
+        return set_error("cudaFuncSetAttribute(max dynamic smem) failed");
   if (getenv("B2P_TRACE")) {
     if (cudaMalloc(&g_trace, sizeof(unsigned long long) * kTraceCap * kTraceCtas * kTraceSlots) != cudaSuccess)
       return set_error("B2P_TRACE: setup of the traced kernel failed");
@@ -895,6 +1073,7 @@ struct GemmKnobs {
   bool few_ctas;      // unset B2P_DENSE_GRIDS: single-wave launches pay a charge per occupied SM
   double cta_penalty; // B2P_CTA_PENALTY: microseconds charged per CTA (default 0.02)
   int max_grid;       // B2P_MAX_GRID: experiment, cap the grid of launches that do not split K (0 = none)
+  bool no_tma_epi;    // B2P_NO_TMA_EPI: every launch keeps the register epilogue (per-thread global loads and stores)
 };
 static const GemmKnobs& gemm_knobs() {
   static const GemmKnobs k = [] {
@@ -907,6 +1086,7 @@ static const GemmKnobs& gemm_knobs() {
     v.few_ctas = getenv("B2P_DENSE_GRIDS") == nullptr;
     v.cta_penalty = getenv("B2P_CTA_PENALTY") ? atof(getenv("B2P_CTA_PENALTY")) : 0.02;
     v.max_grid = getenv("B2P_MAX_GRID") ? atoi(getenv("B2P_MAX_GRID")) : 0;
+    v.no_tma_epi = getenv("B2P_NO_TMA_EPI") != nullptr;
     return v;
   }();
   return k;
@@ -981,6 +1161,7 @@ struct TmaGeom {
   cuuint64_t dims[5], strides[4];
   cuuint32_t box[5];
   CUtensorMapSwizzle swizzle;   // must span exactly one box row (bk * 2 bytes) and match the wgmma descriptors' layout
+  bool f32;                     // fp32 elements (else fp16, or bf16 for bf16 operands)
 };
 static int swizzle_bytes(CUtensorMapSwizzle s) {
   return s == CU_TENSOR_MAP_SWIZZLE_128B ? 128 : s == CU_TENSOR_MAP_SWIZZLE_64B ? 64 : s == CU_TENSOR_MAP_SWIZZLE_32B ? 32 : 0;
@@ -993,10 +1174,48 @@ static int desc_swizzle_bytes(uint64_t desc_hi) {   // layout field [62,64) of t
 // which belong to the launching stream), both tensor maps' geometry, the grid and the dynamic shared memory.
 struct GemmPlan {
   GemmArgs g;
-  TmaGeom ta, tb;
+  TmaGeom ta, tb, tc, tr;   // tc / tr: TMA epilogue output / residual
   int kb_merge, grid;
   size_t smem;
 };
+
+// The epilogue, decided after the tiling and the ring: the TMA epilogue (GemmArgs::tma_epi) for direct mode-0 launches with
+// 16-byte aligned rows whose staging and residual buffers fit in the shared memory the ring leaves, giving up ring stages
+// down to 2 (resident weights: A stages) if needed -- but never an fp16x3 stage: those rings are as deep as their
+// k-blocks allow only just.  Otherwise the register epilogue (epi_store16).
+static void plan_epilogue(const ConvGemm& d, int max_smem, const GemmKnobs& kn, int stage_bytes, GemmPlan* p) {
+  GemmArgs& g = p->g;
+  g.epi_bytes = kEpiStageBytes;
+  const int esz = d.out_f32 ? 4 : 2, cols = 64 / esz;
+  if (kn.no_tma_epi || d.mode != 0 || g.ksplit != 1 || g.park || !g.vec_ok || d.N % (16 / esz) != 0 || g.bn % cols != 0) return;
+  const int out_planes = g.split ? 2 : 1, res_planes = !d.res ? 0 : (g.res_lo ? 2 : 1);
+  const uint32_t epi_buf = out_planes * kEpiPlane, res_buf = res_planes * kEpiPlane;
+  const long long epi_bytes = 2LL * (epi_buf + res_buf);
+  const long long need = (long long)p->smem - kEpiStageBytes + epi_bytes - max_smem;   // bytes the ring must give up
+  if (need > 0) {
+    const long long unit = g.bres ? g.a_slot : stage_bytes;
+    const int give = int((need + unit - 1) / unit);
+    int& ring = g.bres ? g.stagesA : g.stages;
+    if (g.x3 || ring - give < 2) return;
+    ring -= give;
+    p->smem -= size_t(give) * size_t(unit);
+  }
+  p->smem += epi_bytes - kEpiStageBytes;
+  g.tma_epi = 1;
+  g.out_planes = out_planes; g.res_planes = res_planes;
+  g.epi_buf = epi_buf; g.res_buf = res_buf; g.epi_bytes = uint32_t(epi_bytes);
+  const cuuint64_t N = cuuint64_t(d.N), M = cuuint64_t(d.M);
+  const cuuint32_t bc = cuuint32_t(cols);
+  // [hi | lo] pairs: one more dimension of size 2, the lo plane at column offset split / res_lo
+  p->tc = out_planes == 2 ? TmaGeom{3, {N, M, 2}, {cuuint64_t(d.ldc) * esz, cuuint64_t(g.split) * esz}, {bc, kTileM, 2}}
+                          : TmaGeom{2, {N, M}, {cuuint64_t(d.ldc) * esz}, {bc, kTileM}};
+  if (res_planes) {
+    p->tr = res_planes == 2 ? TmaGeom{3, {N, M, 2}, {cuuint64_t(d.ldr) * esz, cuuint64_t(g.res_lo) * esz}, {bc, kTileM, 2}}
+                            : TmaGeom{2, {N, M}, {cuuint64_t(d.ldr) * esz}, {bc, kTileM}};
+  }
+  p->tc.swizzle = p->tr.swizzle = CU_TENSOR_MAP_SWIZZLE_64B;
+  p->tc.f32 = p->tr.f32 = d.out_f32 != 0;
+}
 
 // Plans one launch for a device with num_sms SMs and max_smem bytes of opt-in shared memory per block; makes every
 // host-side rejection of gemm_launch and touches no device state.  have_ws: a split-K workspace slot is available for the
@@ -1185,6 +1404,7 @@ static int plan_gemm(const ConvGemm& d, int num_sms, int max_smem, const GemmKno
   g.vec_ok = ((reinterpret_cast<uintptr_t>(d.out) & 15) == 0) && ((d.ldc * esz) % 16 == 0) &&
              (!d.res || (((reinterpret_cast<uintptr_t>(d.res) & 15) == 0) && ((d.ldr * esz) % 16 == 0))) &&
              (!d.bias || ((reinterpret_cast<uintptr_t>(d.bias) & 15) == 0));
+  plan_epilogue(d, max_smem, kn, stage_bytes, p);
   const int total = g.m_tiles * g.n_tiles * g.ksplit;
   int grid = total < num_sms ? total : num_sms;
   if (kn.max_grid > 0 && grid > kn.max_grid && ksplit == 1) grid = kn.max_grid;
@@ -1193,7 +1413,8 @@ static int plan_gemm(const ConvGemm& d, int num_sms, int max_smem, const GemmKno
 }
 
 static int encode(CUtensorMap* m, int bf16, const TmaGeom& t, const void* base) {
-  return encode(m, bf16, t.rank, base, t.dims, t.strides, t.box, t.swizzle);
+  const CUtensorMapDataType dt = t.f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  return encode(m, dt, t.rank, base, t.dims, t.strides, t.box, t.swizzle);
 }
 
 static void plan_fields(const GemmPlan& p, int* out);
@@ -1211,9 +1432,14 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
   GemmArgs& g = p.g;
   g.ws = slot >= 0 ? g_ws[slot] : nullptr;
   g.counters = slot >= 0 ? g_counters[slot] : nullptr;
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmC{}, tmR{};
   if (int e = encode(&tmA, d.bf16, p.ta, d.A)) return e;
   if (int e = encode(&tmB, d.bf16, p.tb, d.B)) return e;
+  if (g.tma_epi) {
+    if (int e = encode(&tmC, 0, p.tc, d.out)) return e;
+    if (g.res_planes)
+      if (int e = encode(&tmR, 0, p.tr, d.res)) return e;
+  }
   const int grid = p.grid, bn = g.bn, ksplit = g.ksplit;
   const int Ktot = (d.mode == 0) ? d.K : 9 * d.Cin;
   static const bool dbg = getenv("B2P_DEBUG") != nullptr;
@@ -1243,9 +1469,9 @@ int gemm_launch(const ConvGemm& d, cudaStream_t st) {
     }
   }
   GemmKernel kern = nullptr;
-  for (int i = 0; i < kNumBn; ++i) if (kBnCand[i] == bn) kern = kGemmKernels[i];
+  for (int i = 0; i < kNumBn; ++i) if (kBnCand[i] == bn) kern = kGemmKernels[i][g.tma_epi];
   if (!kern) return set_error("gemm: internal error, no kernel instantiation for the chosen N tile");
-  cudaError_t ce = cudaLaunchKernelEx(&cfg, kern, tmA, tmB, g);
+  cudaError_t ce = cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, tmR, g);
   if (ce == cudaSuccess) ce = cudaGetLastError();
   if (ce != cudaSuccess) return set_error(cudaGetErrorString(ce));
   count_launch();
@@ -1286,6 +1512,25 @@ int gemm_plan_host(const ConvGemm& d, int num_sms, int max_smem, int* out) {
   GemmPlan p;
   if (int e = plan_gemm(d, num_sms, max_smem, kn, !(kn.no_split || d.no_split), &p)) return e;
   plan_fields(p, out);
+  return 0;
+}
+
+// Host-only epilogue planner (b2p_gemm_epilogue_plan): see include/b200parse.h for the field order of `out`.
+int gemm_epilogue_plan_host(const ConvGemm& d, int num_sms, int max_smem, int* out) {
+  if (num_sms < 1 || max_smem < 1) return set_error("gemm_plan: num_sms and max_smem must be positive");
+  const GemmKnobs& kn = gemm_knobs();
+  GemmPlan p;
+  if (int e = plan_gemm(d, num_sms, max_smem, kn, !(kn.no_split || d.no_split), &p)) return e;
+  const GemmArgs& g = p.g;
+  auto sat = [](cuuint64_t v) { return int(v > 0x7fffffffULL ? 0x7fffffffULL : v); };
+  const int cols = d.out_f32 ? 16 : 32;
+  const int f[] = {g.tma_epi, g.tma_epi ? cols : 0, g.tma_epi ? g.bn / cols : 0, g.tma_epi ? 2 : 0, g.out_planes,
+                   g.tma_epi && g.res_planes ? 2 : 0, g.res_planes, int(g.epi_bytes), g.stages, g.stagesA, int(p.smem),
+                   p.tc.rank, int(p.tc.box[0]), int(p.tc.box[1]), int(p.tc.box[2]), sat(p.tc.strides[0]), sat(p.tc.strides[1]),
+                   p.tr.rank, int(p.tr.box[0]), int(p.tr.box[1]), int(p.tr.box[2]), sat(p.tr.strides[0]), sat(p.tr.strides[1]),
+                   swizzle_bytes(p.tc.swizzle)};
+  static_assert(sizeof(f) / sizeof(f[0]) == kEpiPlanFields, "b2p_gemm_epilogue_plan field count");
+  for (int i = 0; i < kEpiPlanFields; ++i) out[i] = f[i];
   return 0;
 }
 

@@ -7,7 +7,9 @@ stamps %globaltimer per CTA at the phase boundaries) and prints, per launch, the
 Phases: prologue (barrier init, descriptor prefetch) | dep-wait (griddepcontrol.wait: the previous kernel's
 tail under PDL) | first TMA issued | first stage landed (TMA latency) | first tile's MMAs issued | accumulator ready ->
 epilogue starts | epilogue + remaining tiles | teardown.  `span` = first CTA entry -> last CTA exit; `gap` = this launch's
-first entry minus the previous launch's last exit (negative = overlapped through PDL).
+first entry minus the previous launch's last exit (negative = overlapped through PDL).  `main` / `epi`: one consumer
+thread's time per CTA summed over all of its items, item start -> accumulators ready (MMA main loop with its TMA waits) and
+accumulators ready -> item end (epilogue, split-K reduction); `epi%` = epi / (main + epi) over all CTAs of the launches.
 """
 import ctypes as C
 import os
@@ -52,13 +54,20 @@ def report(stamps, meta, limit=400):
             v = v[(v[:, 0] > 0) & (v[:, 1] > 0)]
             ph.append(float(np.median(v[:, 1] - v[:, 0])) / 1e3 if len(v) else float("nan"))
         key = tuple(int(x) for x in m)
-        a = agg.setdefault(key, [0, 0.0, np.zeros(8), 0.0])
+        a = agg.setdefault(key, [0, 0.0, np.zeros(8), 0.0, 0.0, 0.0])
         a[0] += 1; a[1] += span; a[2] += np.nan_to_num(np.array(ph)); a[3] += 0.0 if gap != gap else gap
+        a[4] += s[ok, 9].sum() / 1e3; a[5] += s[ok, 10].sum() / 1e3
         if i < limit:
             print("%4d %7d %5d %6d %3d %2d %2d %4d | %5.1f %6.1f | " % (*key, span, gap) + " ".join(f"{x:9.2f}" for x in ph))
     print("\nper shape (mean over launches), sorted by total span:")
-    for key, (n, sp, ph, gp) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:40]:
-        print("%4d %7d %5d %6d %3d %2d %2d %4d | n=%3d span %6.1f gap %6.1f | " % (*key, n, sp / n, gp / n) + " ".join(f"{x:9.2f}" for x in ph / n))
+    top = sorted(agg.items(), key=lambda kv: -kv[1][1])
+    for key, (n, sp, ph, gp, mn, ep) in top[:40]:
+        print("%4d %7d %5d %6d %3d %2d %2d %4d | n=%3d span %6.1f gap %6.1f | " % (*key, n, sp / n, gp / n) + " ".join(f"{x:9.2f}" for x in ph / n)
+              + "   epi%% %5.1f" % (100.0 * ep / max(mn + ep, 1e-9)))
+    for k in (20, len(top)):
+        mn = sum(v[4] for _, v in top[:k]); ep = sum(v[5] for _, v in top[:k]); sp = sum(v[1] for _, v in top[:k])
+        print("top %3d shapes: total span %8.1f us, CTA-time main %10.1f us, epi %10.1f us, epi%% %5.1f"
+              % (k, sp, mn, ep, 100.0 * ep / max(mn + ep, 1e-9)))
 
 
 what = sys.argv[1] if len(sys.argv) > 1 else "shapes"
