@@ -117,7 +117,9 @@ int b2p_cbfuse_x3(int nsrc, const void* const* srcs_host, const long long* lds_h
                   long long ldy, long long lol, long long loy, b2p_stream_t stream);
 
 /* ---- detector pre/post-processing ----
- * b2p_letterbox: PIL Image.resize(LANCZOS) + paste on a 114 canvas, ref:util/yolov9.py:73-84 (bit-exact).
+ * b2p_letterbox: PIL Image.resize(LANCZOS) + paste on a 114 canvas, ref:util/yolov9.py:73-84 (bit-exact).  Returns an
+ *                error without launching when a size is < 1 (Pillow raises) or the resized image does not lie inside
+ *                the canvas; b2p_resize_u8 likewise for sizes < 1.
  * b2p_im2col_u8: /255 (ref:util/yolov9.py:85) or CLIP rescale+normalise (ref:util/utils.py:121) via `lut` [3][256]
  *                + im2col of the 3-channel stem conv; split != 0 writes the fp16x3 layout.
  * b2p_yolo_decode: ref:util/yolov9.py:89-108 (_decode) and :123-129 (class max, strict conf filter, un-letterbox).

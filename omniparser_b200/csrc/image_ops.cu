@@ -295,6 +295,10 @@ int b2p_lanczos_coeffs_host(int in_size, int out_size, int* ksize, int* bounds /
 // (Wr, Hr) = resized size, pasted at (pad_l, pad_t); ref:util/yolov9.py:73-84.
 int b2p_letterbox(const unsigned char* src, int B, int H, int W, int Wr, int Hr, int Tw, int Th, int pad_l, int pad_t,
                   unsigned char* tmp, unsigned char* canvas, cudaStream_t st) {
+  // Pillow raises on an empty resize; an empty coefficient table would otherwise leave an all-114 canvas
+  if (W < 1 || H < 1 || Wr < 1 || Hr < 1) return set_error("letterbox: source and resized sizes must be >= 1");
+  if (pad_l < 0 || pad_t < 0 || pad_l + Wr > Tw || pad_t + Hr > Th)
+    return set_error("letterbox: the resized image must lie inside the canvas");
   const unsigned char* hsrc = src;
   int hW = W;
   if (Wr != W) {   // Pillow skips a pass whose size does not change
@@ -318,6 +322,7 @@ int b2p_letterbox(const unsigned char* src, int B, int H, int W, int Wr, int Hr,
 int b2p_resize_u8(const unsigned char* src, int B, int H, int W, int Wr, int Hr, int filter, unsigned char* tmp,
                   unsigned char* out, cudaStream_t st) {
   if (filter != 0 && filter != 1) return set_error("resize_u8: filter must be 0 (LANCZOS) or 1 (BICUBIC)");
+  if (W < 1 || H < 1 || Wr < 1 || Hr < 1) return set_error("resize_u8: source and resized sizes must be >= 1");
   const unsigned char* hsrc = src;
   int hW = W;
   if (Wr != W) {

@@ -41,6 +41,8 @@ def _geometry(w: int, h: int, imgsz):
     th = ((int(th) + 31) // 32) * 32
     scale = min(tw / w, th / h)
     rw, rh = int(w * scale), int(h * scale)
+    if rw < 1 or rh < 1:   # Pillow's resize raises the same (e.g. 641 x 1 at imgsz 640 resizes to 640 x 0)
+        raise ValueError(f"height and width must be > 0: a {w} x {h} image resizes to {rw} x {rh} at imgsz {imgsz}")
     return tw, th, scale, rw, rh, (tw - rw) // 2, (th - rh) // 2
 
 
