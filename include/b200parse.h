@@ -33,6 +33,22 @@ int b2p_abi_version(void);
  * accumulator issued, first epilogue start, last epilogue end, exit), meta [n][8] = {mode, M, N, K, bn, ksplit, x3, grid}. */
 int b2p_trace_read(unsigned long long* stamps, int* meta, int max_launches);
 
+/* ---- streams and split-K workspace slots (host only) ----
+ * Split-K GEMM/conv launches park partial tiles in a workspace slot owned by the launching stream (under graph capture: the
+ * capture stream, whose slot the graph bakes in); a stream claims one of 24 slots at its first GEMM/conv launch.  Streams that
+ * may run concurrently must therefore be distinct handles.
+ * b2p_stream_create: a new non-blocking stream on the current device (cudaStreamCreateWithFlags), outside any pool.
+ * b2p_stream_destroy: destroys a stream and releases its slot; the caller ensures the stream is idle and that no graph
+ *   captured on it is replayed afterwards.
+ * b2p_ws_slot: the slot the stream owns, or -1; never claims one.
+ * b2p_ws_audit: synchronises the device, then nonzero_host[i] (i < max_slots) = the number of non-zero arrival-counter words
+ *   of slot i, or -1 if no stream owns it; returns the number of slots (24).  A completed split-K launch leaves its counters
+ *   at zero, so with the device idle every owned slot should report 0.  For tests and debugging. */
+int b2p_stream_create(b2p_stream_t* out);
+int b2p_stream_destroy(b2p_stream_t st);
+int b2p_ws_slot(b2p_stream_t st);
+int b2p_ws_audit(int* nonzero_host, int max_slots);
+
 /* ---- dense contractions (wgmma + TMA), ref:util/yolov9.py:120-121 and ref:util/utils.py:125 ----
  * flags: bit0 operands bf16 (else fp16) | bit1 output fp32 (else fp16) | bit2 fp16 output in the "fp16x3" operand
  * layout [hi(N) | lo(N)] (ldc >= 2N) | bit3 fp16x3 OPERANDS: A rows [hi(K) | lo(K)] (lda >= 2K; conv: pixels

@@ -24,6 +24,10 @@ PROTOTYPES = {
     "b2p_launch_count": (i64, []),
     "b2p_trace_read": (i32, [vp, vp, i32]),
     "b2p_abi_version": (i32, []),
+    "b2p_stream_create": (i32, [vp]),
+    "b2p_stream_destroy": (i32, [vp]),
+    "b2p_ws_slot": (i32, [vp]),
+    "b2p_ws_audit": (i32, [vp, i32]),
     "b2p_gemm": (i32, [vp, i64, vp, i32, i32, i32, vp, i64, vp, vp, i64, i32, i32, vp]),
     "b2p_conv3x3": (i32, [vp, i64, i32, i32, i32, i32, i32, vp, i32, vp, i64, vp, vp, i64, i32, i32, vp]),
     "b2p_gemm_planes": (i32, [vp, i64, vp, i32, i32, i32, vp, i64, vp, vp, i64, i32, i32, i64, i64, i64, vp]),

@@ -55,6 +55,12 @@ int b2p_abi_version(void) { return 2; }
 // Debugging aid (B2P_TRACE=1): per-CTA phase timestamps of the traced GEMM launches, see gemm_wgmma.cu::trace_read.
 int b2p_trace_read(unsigned long long* stamps, int* meta, int max_launches) { return trace_read(stamps, meta, max_launches); }
 
+// Streams and split-K workspace slots (see include/b200parse.h).
+int b2p_stream_create(cudaStream_t* out) { return stream_create(out); }
+int b2p_stream_destroy(cudaStream_t st) { return stream_destroy(st); }
+int b2p_ws_slot(cudaStream_t st) { return ws_slot(st); }
+int b2p_ws_audit(int* nonzero_host, int max_slots) { return ws_audit(nonzero_host, max_slots); }
+
 // C[M,N] = act(A[M,K] * B[N,K]^T + bias) (+ residual); A, B fp16 (bf16 if flags&1); out fp16 or fp32 (flags&2);
 // flags&4: fp16 output in the fp16x3 operand layout [hi(N) | lo(N)] (ldc >= 2N).
 // flags&8: fp16x3 operands: A rows [hi(K) | lo(K)] (lda >= 2K), B rows [hi(K) | lo(K)]; K is the logical reduction size.

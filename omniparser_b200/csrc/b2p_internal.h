@@ -63,6 +63,11 @@ int gemm_last_plan(int* out);
 static constexpr int kEpiPlanFields = 24;
 int gemm_epilogue_plan_host(const ConvGemm& d, int num_sms, int max_smem, int* out);   // the same fields for the calling thread's most recent launch
 int trace_read(unsigned long long* stamps, int* meta, int max_launches);   // B2P_TRACE=1 debugging aid
+// streams outside torch's pool and the split-K workspace slot each one owns (gemm_wgmma.cu)
+int stream_create(cudaStream_t* out);
+int stream_destroy(cudaStream_t st);
+int ws_slot(cudaStream_t st);
+int ws_audit(int* nonzero_host, int max_slots);
 
 // Second-version SIMT kernels of the caption encoder (florence_simt.cu).  Return 0 = launched, 1 = shape not covered (the caller
 // falls back to the first-version kernel), < 0 = error (message recorded).

@@ -995,18 +995,25 @@ static int encode(CUtensorMap* m, CUtensorMapDataType dtype, int rank, const voi
 
 static int g_num_sms = 0;
 // Split-K scratch is per stream (two streams may run split-K GEMMs concurrently): a few slots are allocated up
-// front (never inside a graph capture) and handed to streams in order of first use.
+// front (never inside a graph capture) and handed to streams at their first launch; a slot goes back to the free list when
+// its stream is destroyed through stream_destroy.  A graph bakes in the slot of the stream it was captured on.
 static constexpr int kWsSlots = 24;
 static float* g_ws[kWsSlots] = {};
 static int* g_counters[kWsSlots] = {};
 static cudaStream_t g_ws_owner[kWsSlots] = {};
-static int g_ws_used = 0;
+static bool g_ws_taken[kWsSlots] = {};
 static std::mutex g_ws_mu;
+static int ws_slot_locked(cudaStream_t st) {
+  for (int i = 0; i < kWsSlots; ++i)
+    if (g_ws_taken[i] && g_ws_owner[i] == st) return i;
+  return -1;
+}
 static int ws_slot_for(cudaStream_t st) {
   std::lock_guard<std::mutex> lk(g_ws_mu);
-  for (int i = 0; i < g_ws_used; ++i)
-    if (g_ws_owner[i] == st) return i;
-  if (g_ws_used < kWsSlots) { g_ws_owner[g_ws_used] = st; return g_ws_used++; }
+  const int have = ws_slot_locked(st);
+  if (have >= 0) return have;
+  for (int i = 0; i < kWsSlots; ++i)
+    if (!g_ws_taken[i]) { g_ws_taken[i] = true; g_ws_owner[i] = st; return i; }
   return -1;   // more concurrent streams than slots: the caller disables split-K for this launch
 }
 static constexpr size_t kWsBytes = size_t(64) << 20;     // split-K partial tiles (per slot)
@@ -1555,6 +1562,49 @@ int trace_read(unsigned long long* stamps, int* meta, int max_launches) {
   cudaMemset(g_trace, 0, sizeof(unsigned long long) * per * kTraceCap);
   g_trace_n = 0;
   return n;
+}
+
+// ------------------------------------------------------------------------ streams and their split-K workspace slots
+int stream_create(cudaStream_t* out) {
+  if (!out) return set_error("stream_create: out is null");
+  if (int e = bind_device()) return e;
+  if (cudaStreamCreateWithFlags(out, cudaStreamNonBlocking) != cudaSuccess) return set_error("cudaStreamCreateWithFlags failed");
+  return 0;
+}
+
+int stream_destroy(cudaStream_t st) {
+  if (!st) return set_error("stream_destroy: the default stream is not destroyed");
+  // the slot is released under the lock before the handle can be reused by a new stream
+  std::lock_guard<std::mutex> lk(g_ws_mu);
+  const int i = ws_slot_locked(st);
+  if (i >= 0) { g_ws_taken[i] = false; g_ws_owner[i] = nullptr; }
+  if (cudaStreamDestroy(st) != cudaSuccess) return set_error("cudaStreamDestroy failed");
+  return 0;
+}
+
+int ws_slot(cudaStream_t st) {
+  std::lock_guard<std::mutex> lk(g_ws_mu);
+  return ws_slot_locked(st);
+}
+
+// Every split-K launch leaves its tiles' arrival counters at zero (the last CTA of a tile resets them), so with the device
+// idle a non-zero counter word is a launch that did not complete its reduction, or two launches that shared a slot.
+int ws_audit(int* nonzero_host, int max_slots) {
+  if (!nonzero_host && max_slots > 0) return set_error("ws_audit: nonzero_host is null");
+  if (int e = bind_device()) return e;
+  if (cudaDeviceSynchronize() != cudaSuccess) return set_error("ws_audit: cudaDeviceSynchronize failed");
+  static int words[2 * kMaxCounterTiles];
+  std::lock_guard<std::mutex> lk(g_ws_mu);
+  for (int i = 0; i < kWsSlots && i < max_slots; ++i) {
+    nonzero_host[i] = -1;
+    if (!g_ws_taken[i]) continue;
+    if (cudaMemcpy(words, g_counters[i], sizeof words, cudaMemcpyDeviceToHost) != cudaSuccess)
+      return set_error("ws_audit: counter copy failed");
+    int n = 0;
+    for (int w = 0; w < 2 * kMaxCounterTiles; ++w) n += words[w] != 0;
+    nonzero_host[i] = n;
+  }
+  return kWsSlots;
 }
 
 }  // namespace b2p

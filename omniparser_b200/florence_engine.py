@@ -514,7 +514,7 @@ class FlorencePlan:
         # reading them, so those steps replay a graph WITHOUT the LM head (51290 x 768, the largest GEMM of the step).  The
         # decoder layers still run: the KV cache of the step is needed by the following steps.
         return dict(idx=idx, r0=r0, r1=r1, ops=ops_, pick=pick, step=step, n_unf=n_unf, graph=None, graph_forced=None,
-                    stream=torch.cuda.Stream(device=self.dev), full=ops_ + pick_ops + [lambda: ops.step_advance(step)],
+                    stream=ops.role_stream(f"{self.tag}_part{idx}", self.dev), full=ops_ + pick_ops + [lambda: ops.step_advance(step)],
                     full_forced=ops_[:-1] + pick_ops + [lambda: ops.step_advance(step)])
 
     def _alloc_beam_state(self, tmax):
@@ -563,7 +563,7 @@ class FlorencePlan:
             torch.cuda.current_stream().synchronize()
             g = torch.cuda.CUDAGraph()
             with ops.CAPTURE_LOCK:   # one capture at a time across the pipeline's threads
-                with torch.cuda.graph(g, stream=ops.capture_stream(tag, self.dev), capture_error_mode="thread_local"):
+                with torch.cuda.graph(g, stream=ops.role_stream(tag, self.dev), capture_error_mode="thread_local"):
                     for f in lst:
                         f()
             if isinstance(holder, dict):

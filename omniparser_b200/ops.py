@@ -14,17 +14,44 @@ import torch
 from . import _lib
 
 ACT_NONE, ACT_SILU, ACT_GELU = 0, 1, 2
-_CAPTURE_STREAMS = {}
+_ROLE_STREAMS = {}
+_ROLE_LOCK = threading.Lock()
 CAPTURE_LOCK = threading.RLock()   # one CUDA-graph capture at a time across the pipeline's threads
 
 
-def capture_stream(tag, device):
-    """One capture stream per engine: split-K scratch is keyed by stream, and graphs of different engines may replay
-    concurrently on different streams."""
-    key = (tag, str(device))
-    if key not in _CAPTURE_STREAMS:
-        _CAPTURE_STREAMS[key] = torch.cuda.Stream(device=device)
-    return _CAPTURE_STREAMS[key]
+def _stream_device(device):
+    """the CUDA device (with its index) whose streams serve ``device``, or None for a device without CUDA streams"""
+    dev = torch.device(device)
+    if dev.type != "cuda":
+        return None
+    return dev if dev.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def role_stream(tag, device):
+    """The stream of one role, created once per (role, device): the capture stream of an engine ('yolo', 'florence{lane}',
+    'florence{lane}_dec{part}'), a pipeline stage ('det', 'cap{lane}'), a decode chain ('florence{lane}_part{p}').
+
+    Split-K scratch is keyed by the launching stream (the capture stream, for a graph), and streams of different roles may
+    run concurrently, so every role needs its own handle.  torch's streams cannot promise that: torch.cuda.Stream hands out
+    a round-robin pool of 32 streams per device, and the 33rd request returns the first one again.  These streams come from
+    b2p_stream_create instead, outside the pool, and are never destroyed.  Caching by role keeps the number of split-K
+    workspace slots in use bounded: no new stream per parser or per plan.
+
+    A device without CUDA streams (plans built on the CPU for host-side dry runs) has no roles to separate: the caller's
+    current stream is returned."""
+    dev = _stream_device(device)
+    if dev is None:
+        return torch.cuda.current_stream()
+    key = (tag, str(dev))
+    with _ROLE_LOCK:
+        s = _ROLE_STREAMS.get(key)
+        if s is None:
+            h = C.c_void_p(0)
+            with torch.cuda.device(dev):
+                _lib.check(_lib.lib().b2p_stream_create(C.byref(h)))
+            s = torch.cuda.ExternalStream(h.value, device=dev)
+            _ROLE_STREAMS[key] = s
+        return s
 
 
 GRAPH_LAUNCHES = [0]   # kernels replayed through CUDA graphs (the C-side counter only sees direct launches)

@@ -12,6 +12,8 @@ from typing import List, Sequence, Tuple
 import numpy as np
 import torch
 
+from . import ops
+
 # record capacity per screenshot: every detected icon can be captioned (max_det = 300, ref:util/yolov9.py:131 `[:max_det]`;
 # the reference captions ALL of them, in chunks of batch_size, ref:util/utils.py:116) and the element list holds the icons
 # plus the OCR boxes that survive the overlap filter.  Exceeding a capacity raises: a truncated record would make rank 0
@@ -87,7 +89,7 @@ class GatherPipe:
         self.rank, self.world, self.dev, self.T, self.keep = rank, world, torch.device(device), max_new_tokens, keep
         self.shape = (batch, record_width(max_new_tokens))
         self.cuda = self.dev.type == "cuda"
-        self.stream = torch.cuda.Stream(device=self.dev) if self.cuda else None
+        self.stream = ops.role_stream("gather", self.dev) if self.cuda else None
         self.free: "queue.Queue" = queue.Queue()
         self.work: "queue.Queue" = queue.Queue()
         self.received: list = []

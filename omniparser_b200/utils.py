@@ -217,15 +217,16 @@ class PipelinedParser:
         self.model, self.cmp = model, caption_model_processor
         self.conf, self.iou_thr, self.imgsz, self.T, self.prompt = BOX_TRESHOLD, iou_threshold, imgsz, max_new_tokens, list(prompt_ids)
         dev = model.device
-        self.s_det = torch.cuda.Stream(device=dev)
-        self.s_cap = torch.cuda.Stream(device=dev)
+        # role streams (ops.role_stream): one per stage and lane, shared by every parser of the device, never aliased
+        self.s_det = ops.role_stream("det", dev)
+        self.s_cap = ops.role_stream("cap0", dev)
         self.timings = ParseTimings(detect_wait_s=0.0, glue_s=0.0, caption_s=0.0, n_boxes=0, n_crops=0, batches=0)
         from concurrent.futures import ThreadPoolExecutor
         self._pool = ThreadPoolExecutor(max_workers=1, thread_name_prefix="b2p-submit")   # host staging copy off the main thread
         # caption stage: CAPTION_LANES batches in flight, each on its own stream with its own plan instance -- the
         # latency-bound decode steps of one batch fill the SMs the other batch's encoder leaves idle, and vice versa
         self.lanes = max(1, int(caption_lanes))
-        self.s_caps = [self.s_cap] + [torch.cuda.Stream(device=dev) for _ in range(self.lanes - 1)]
+        self.s_caps = [self.s_cap] + [ops.role_stream(f"cap{i}", dev) for i in range(1, self.lanes)]
         # one single-worker executor PER LANE: two batches of the same lane share a plan and a stream, so they must
         # never be in flight together (a shared pool lets batch i+2 start on lane 0 while batch i still decodes there)
         self._cap_pools = [ThreadPoolExecutor(max_workers=1, thread_name_prefix=f"b2p-caption{i}") for i in range(self.lanes)]

@@ -379,7 +379,7 @@ class YoloPlan:
                 f()
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
-            with ops.CAPTURE_LOCK, torch.cuda.graph(g, stream=ops.capture_stream('yolo', self.dev), capture_error_mode="thread_local"):
+            with ops.CAPTURE_LOCK, torch.cuda.graph(g, stream=ops.role_stream('yolo', self.dev), capture_error_mode="thread_local"):
                 for f in self.ops:
                     f()
             self.graph = g
