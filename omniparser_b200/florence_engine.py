@@ -196,8 +196,9 @@ class FlorencePlan:
         self.v3 = not os.environ.get("B2P_NO_SIMT_V3")
         # B2P_GEMM_LN=1: decoder out-proj / cross out-proj / fc2 as park-only split-K GEMM + one reduce/LayerNorm kernel
         # (b2p_gemm_ln) instead of GEMM with in-kernel split-K reduction + LayerNorm launch.  Bit-identical; the kernel boundary
-        # costs about what the in-kernel wait cost, so it stays opt-in.
-        self.fuse_ln = bool(os.environ.get("B2P_GEMM_LN"))
+        # costs about what the in-kernel wait cost, so it stays opt-in.  The park-only GEMM needs split-K, so B2P_NO_SPLITK
+        # (any value, as the planner reads it) keeps the unfused pair.
+        self.fuse_ln = bool(os.environ.get("B2P_GEMM_LN")) and "B2P_NO_SPLITK" not in os.environ
         self.warmed = False
         import threading
         self.lock = threading.Lock()

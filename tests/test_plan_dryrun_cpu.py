@@ -156,6 +156,24 @@ def test_gemm_ln_opt_in(rec, florence, monkeypatch):
     assert len(names) == 71 - 18 and names.count("b2p_gemm_ln") == 18 and names.count("b2p_layernorm") == 1
 
 
+@pytest.mark.parametrize("value", ["1", ""])
+def test_gemm_ln_not_chosen_without_split_k(rec, florence, monkeypatch, value):
+    """B2P_GEMM_LN=1 with B2P_NO_SPLITK set (to anything: the planner tests presence): the planner refuses park-only
+    GEMMs, so the decode step keeps its GEMM + LayerNorm pairs instead of b2p_gemm_ln launches that would raise"""
+    from omniparser_b200.florence_engine import FlorencePlan, FlorenceWeights
+    monkeypatch.setenv("B2P_GEMM_LN", "1")
+    monkeypatch.setenv("B2P_NO_SPLITK", value)
+    w = FlorenceWeights(florence.state_dict(), torch.device("cpu"), FS.GEN, "fp16x3")
+    p = FlorencePlan(w, 2, 4, FS.PROMPT_IDS, use_graph=False, size=64)
+    assert not p.fuse_ln
+    p.encode()
+    n_enc = len(rec.calls)
+    p.reset_decode(2)
+    p.decode_step()
+    names = [c[0] for c in rec.calls[n_enc:]]
+    assert len(names) == 71 and "b2p_gemm_ln" not in names and names.count("b2p_layernorm") == 19
+
+
 def test_florence_plan_768(rec, florence):
     from omniparser_b200.florence_engine import FlorencePlan, FlorenceWeights
     w = FlorenceWeights(florence.state_dict(), torch.device("cpu"), FS.GEN, "fp16x3")
