@@ -144,6 +144,25 @@ int b2p_cbfuse_x3(int nsrc, const void* const* srcs_host, const long long* lds_h
 int b2p_lanczos_coeffs_host(int in_size, int out_size, int* ksize_host, int* bounds_host, int* kk_host, int kk_capacity);
 int b2p_letterbox(const unsigned char* src, int B, int H, int W, int Wr, int Hr, int Tw, int Th, int pad_l, int pad_t,
                   unsigned char* tmp, unsigned char* canvas, b2p_stream_t stream);
+/* Ragged letterbox: b2p_letterbox for a batch of screenshots of DIFFERENT sizes onto one canvas (Tw, Th), in at most two
+ * launches, with the same arithmetic (ref:util/yolov9.py:73-84 per image; bit-exact).
+ * b2p_letterbox_batch_plan_host (host only, no device touched): geom_host [B][6] = per image (H, W, Wr, Hr, pad_l, pad_t) ->
+ *   desc_host [B][12] int64 per image: 0 byte offset of the image in the flat src buffer ([H][W][3], images back to back),
+ *   1 byte offset of its horizontal-pass output in tmp ([H][Wr][3], -1 when Wr == W: Pillow skips that pass), 2-7 H, W,
+ *   Wr, Hr, pad_l, pad_t, 8 / 9 element offset in the table buffer and ksize of the horizontal table (-1 / -1 when Wr == W),
+ *   10 / 11 the same for the vertical table (-1 / -1 when Hr == H);
+ *   tables_host: int32 tables ([out][2] bounds, then [out][ksize] 22-bit weights), one per distinct (in, out) pair of the
+ *   batch, from a bounded host cache (256 pairs, least recently used evicted);
+ *   sizes_host [3] = table ints, tmp bytes, src bytes the batch needs.
+ *   tables_host == NULL is a size query: only sizes_host is written.  Refused before anything is written: B outside
+ *   [1, 65535], a size < 1, a resized image outside the canvas, tables_capacity (ints) < the tables' size.
+ * b2p_letterbox_batch: desc_host is the plan's descriptor array on the host (validated, and read for the launch
+ *   geometry), desc / tables its device copies; src / tmp are the flat buffers the descriptors address, canvas
+ *   [B][Th][Tw][3].  No allocation and no synchronous copy. */
+int b2p_letterbox_batch_plan_host(int B, const int* geom_host, int Tw, int Th, long long* desc_host, int* tables_host,
+                                  long long tables_capacity, long long* sizes_host);
+int b2p_letterbox_batch(const unsigned char* src, int B, const long long* desc_host, const long long* desc, const int* tables,
+                        int Tw, int Th, unsigned char* tmp, unsigned char* canvas, b2p_stream_t stream);
 /* Pillow-exact u8 resize, filter 0 LANCZOS / 1 BICUBIC (CLIP processor resample=3, ref:util/utils.py:123 CPU branch) */
 int b2p_resize_u8(const unsigned char* src, int B, int H, int W, int Wr, int Hr, int filter, unsigned char* tmp,
                   unsigned char* out, b2p_stream_t stream);

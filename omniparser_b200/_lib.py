@@ -48,6 +48,8 @@ PROTOTYPES = {
     "b2p_batched_nms": (i32, [vp, vp, vp, vp, i32, i32, f64, i32, vp, vp, vp, vp, vp, vp, vp]),
     "b2p_lanczos_coeffs_host": (i32, [i32, i32, C.POINTER(i32), vp, vp, i32]),
     "b2p_letterbox": (i32, [vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
+    "b2p_letterbox_batch_plan_host": (i32, [i32, vp, i32, i32, vp, vp, i64, vp]),
+    "b2p_letterbox_batch": (i32, [vp, i32, vp, vp, vp, i32, i32, vp, vp, vp]),
     "b2p_resize_u8": (i32, [vp, i32, i32, i32, i32, i32, i32, vp, vp, vp]),
     "b2p_im2col3x3": (i32, [vp, i64, i32, i32, i32, i32, i32, i32, vp, vp]),
     "b2p_im2col_u8": (i32, [vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, vp]),

@@ -9,6 +9,10 @@
 #include "b2p_internal.h"
 #include <cuda_fp16.h>
 #include <math.h>
+#include <stdio.h>
+#include <string.h>
+#include <algorithm>
+#include <list>
 #include <vector>
 #include <map>
 #include <mutex>
@@ -108,6 +112,21 @@ __device__ __forceinline__ unsigned char clip8(int v) {
   return (unsigned char)(v < 0 ? 0 : (v > 255 ? 255 : v));
 }
 
+// One output pixel of a Pillow 8-bit pass: cnt taps of 22-bit weights k over the RGB pixels s, s + step, ...; the
+// accumulators start at the rounding half (1 << 21) and the result is clipped to u8.  Every LANCZOS / BICUBIC pass below
+// (one-size and batched, horizontal and vertical) goes through this, so their arithmetic cannot drift apart.
+template <typename Step>
+__device__ __forceinline__ void fir_px(const unsigned char* __restrict__ s, Step step, const int* __restrict__ k, int cnt,
+                                       unsigned char* __restrict__ d) {
+  int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+  for (int t = 0; t < cnt; ++t) {
+    const int w = k[t];
+    const unsigned char* p = s + t * step;
+    a0 += p[0] * w; a1 += p[1] * w; a2 += p[2] * w;
+  }
+  d[0] = clip8(a0); d[1] = clip8(a1); d[2] = clip8(a2);
+}
+
 // horizontal pass: src [B][H][W][3] -> tmp [B][H][Wo][3]
 __global__ void lanczos_h_kernel(const unsigned char* __restrict__ src, int B, int H, int W, int Wo,
                                  const int* __restrict__ bounds, const int* __restrict__ kk, int ksize,
@@ -117,15 +136,7 @@ __global__ void lanczos_h_kernel(const unsigned char* __restrict__ src, int B, i
     const int xo = int(i % Wo);
     const long long row = i / Wo;
     const int xmin = bounds[2 * xo], cnt = bounds[2 * xo + 1];
-    const int* k = kk + (long long)xo * ksize;
-    const unsigned char* s = src + (row * W + xmin) * 3;
-    int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
-    for (int x = 0; x < cnt; ++x) {
-      const int w = k[x];
-      a0 += s[3 * x] * w; a1 += s[3 * x + 1] * w; a2 += s[3 * x + 2] * w;
-    }
-    unsigned char* d = tmp + i * 3;
-    d[0] = clip8(a0); d[1] = clip8(a1); d[2] = clip8(a2);
+    fir_px(src + (row * W + xmin) * 3, 3, kk + (long long)xo * ksize, cnt, tmp + i * 3);
   }
 }
 
@@ -148,16 +159,104 @@ __global__ void lanczos_v_paste_kernel(const unsigned char* __restrict__ tmp, in
       continue;
     }
     const int ymin = bounds[2 * yo], cnt = bounds[2 * yo + 1];
-    const int* k = kk + (long long)yo * ksize;
-    const unsigned char* s = tmp + (((long long)b * H + ymin) * Wo + xo) * 3;
-    int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
-    for (int t = 0; t < cnt; ++t) {
-      const int w = k[t];
-      const unsigned char* p = s + (long long)t * Wo * 3;
-      a0 += p[0] * w; a1 += p[1] * w; a2 += p[2] * w;
-    }
-    d[0] = clip8(a0); d[1] = clip8(a1); d[2] = clip8(a2);
+    fir_px(tmp + (((long long)b * H + ymin) * Wo + xo) * 3, (long long)Wo * 3, kk + (long long)yo * ksize, cnt, d);
   }
+}
+
+// ----------------------------------------------------------------------------------------- ragged letterbox
+// A batch of screenshots of different sizes onto one canvas size.  desc [B][kLbDesc] (int64, include/b200parse.h):
+// byte offsets of image b in the flat src / tmp buffers, its geometry, and the element offsets of its horizontal /
+// vertical tables in the packed int32 table buffer ([out][2] bounds, then [out][ksize] weights), -1 for a skipped pass.
+enum { kLbSrc, kLbTmp, kLbH, kLbW, kLbWr, kLbHr, kLbPadL, kLbPadT, kLbHTab, kLbHK, kLbVTab, kLbVK, kLbDesc };
+
+// horizontal pass of every image that needs one: grid (chunks, image); image b: src [H][W][3] -> tmp [H][Wr][3]
+__global__ void lanczos_h_batch_kernel(const unsigned char* __restrict__ src, const long long* __restrict__ desc,
+                                       const int* __restrict__ tables, unsigned char* __restrict__ tmp) {
+  const long long* d = desc + (long long)blockIdx.y * kLbDesc;
+  const long long htab = d[kLbHTab];
+  if (htab < 0) return;
+  const int W = int(d[kLbW]), Wo = int(d[kLbWr]), ksize = int(d[kLbHK]);
+  const long long n = d[kLbH] * Wo;
+  const unsigned char* s = src + d[kLbSrc];
+  unsigned char* t = tmp + d[kLbTmp];
+  const int* bounds = tables + htab;
+  const int* kk = bounds + 2LL * Wo;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int xo = int(i % Wo);
+    const long long row = i / Wo;
+    const int xmin = bounds[2 * xo], cnt = bounds[2 * xo + 1];
+    fir_px(s + (row * W + xmin) * 3, 3, kk + (long long)xo * ksize, cnt, t + i * 3);
+  }
+}
+
+// vertical pass + paste: grid (chunks, image); image b's rows of width Wr come from tmp when it had a horizontal pass,
+// else straight from src (Wr == W) -> canvas [b][Th][Tw][3] at (pad_l, pad_t), 114 elsewhere
+__global__ void lanczos_v_paste_batch_kernel(const unsigned char* __restrict__ src, const long long* __restrict__ desc,
+                                             const int* __restrict__ tables, const unsigned char* __restrict__ tmp, int Tw,
+                                             int Th, unsigned char* __restrict__ canvas) {
+  pdl_wait();   // PDL: inputs come from the previous kernel in the stream
+  const long long* d = desc + (long long)blockIdx.y * kLbDesc;
+  const int Wo = int(d[kLbWr]), Ho = int(d[kLbHr]), pad_l = int(d[kLbPadL]), pad_t = int(d[kLbPadT]);
+  const long long vtab = d[kLbVTab];
+  const int ksize = int(d[kLbVK]);
+  const unsigned char* rows = d[kLbHTab] >= 0 ? tmp + d[kLbTmp] : src + d[kLbSrc];
+  const int* bounds = vtab >= 0 ? tables + vtab : nullptr;
+  const int* kk = vtab >= 0 ? bounds + 2LL * Ho : nullptr;
+  const long long n = (long long)Th * Tw;
+  unsigned char* out = canvas + (long long)blockIdx.y * n * 3;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int x = int(i % Tw);
+    const int y = int(i / Tw);
+    unsigned char* o = out + i * 3;
+    const int xo = x - pad_l, yo = y - pad_t;
+    if (xo < 0 || xo >= Wo || yo < 0 || yo >= Ho) { o[0] = o[1] = o[2] = 114; continue; }
+    if (!bounds) {   // no vertical resample needed (Ho == H)
+      const unsigned char* s = rows + ((long long)yo * Wo + xo) * 3;
+      o[0] = s[0]; o[1] = s[1]; o[2] = s[2];
+      continue;
+    }
+    const int ymin = bounds[2 * yo], cnt = bounds[2 * yo + 1];
+    fir_px(rows + ((long long)ymin * Wo + xo) * 3, (long long)Wo * 3, kk + (long long)yo * ksize, cnt, o);
+  }
+}
+
+// Host-side cache of packed tables ([out][2] bounds | [out][ksize] weights) per (in, out) LANCZOS pair, least recently
+// used first out, so a server that sees recurring screenshot sizes computes each table once.
+struct PackedTable { int ksize; std::vector<int> data; };
+static std::mutex g_lb_mu;
+static std::list<std::pair<std::pair<int, int>, PackedTable>> g_lb_lru;   // most recently used first
+static constexpr size_t kLbCacheEntries = 256;
+
+static PackedTable lb_table(int in, int out) {
+  std::lock_guard<std::mutex> lk(g_lb_mu);
+  const auto key = std::make_pair(in, out);
+  for (auto it = g_lb_lru.begin(); it != g_lb_lru.end(); ++it)
+    if (it->first == key) {
+      g_lb_lru.splice(g_lb_lru.begin(), g_lb_lru, it);
+      return it->second;
+    }
+  std::vector<int> bounds, kk;
+  PackedTable t;
+  host_lanczos_coeffs(in, out, &t.ksize, bounds, kk);
+  t.data = std::move(bounds);
+  t.data.insert(t.data.end(), kk.begin(), kk.end());
+  g_lb_lru.emplace_front(key, t);
+  if (g_lb_lru.size() > kLbCacheEntries) g_lb_lru.pop_back();
+  return t;
+}
+
+static int lb_check_geometry(long long H, long long W, long long Wr, long long Hr, long long pad_l, long long pad_t, int Tw,
+                             int Th, const char* who) {
+  char msg[160];
+  if (W < 1 || H < 1 || Wr < 1 || Hr < 1) {
+    snprintf(msg, sizeof msg, "%s: source and resized sizes must be >= 1", who);
+    return set_error(msg);
+  }
+  if (pad_l < 0 || pad_t < 0 || pad_l + Wr > Tw || pad_t + Hr > Th) {
+    snprintf(msg, sizeof msg, "%s: the resized image must lie inside the canvas", who);
+    return set_error(msg);
+  }
+  return 0;
 }
 
 // ----------------------------------------------------------------------------------------- im2col
@@ -314,6 +413,81 @@ int b2p_letterbox(const unsigned char* src, int B, int H, int W, int Wr, int Hr,
     if (int e = get_coeffs(H, Hr, &cv)) return e;
   launch_pdl(lanczos_v_paste_kernel, dim3(grid_for((long long)B * Th * Tw, 256)), dim3(256), 0, st, hsrc, B, H, hW, Hr, cv.d_bounds, cv.d_kk, cv.ksize,
                                                                               Tw, Th, pad_l, pad_t, canvas);
+  B2P_CHECK_LAUNCH();
+  return 0;
+}
+
+// Host only: the descriptors, packed tables and buffer sizes of one ragged letterbox batch (include/b200parse.h).
+int b2p_letterbox_batch_plan_host(int B, const int* geom_host, int Tw, int Th, long long* desc_host, int* tables_host,
+                                  long long tables_capacity, long long* sizes_host) {
+  if (B < 1 || B > 65535) return set_error("letterbox_batch_plan: B must be in [1, 65535]");
+  for (int b = 0; b < B; ++b) {
+    const int* g = geom_host + 6LL * b;
+    if (int e = lb_check_geometry(g[0], g[1], g[2], g[3], g[4], g[5], Tw, Th, "letterbox_batch_plan")) return e;
+  }
+  // tables: one copy per distinct (in, out) pair of the batch
+  std::vector<long long> desc(size_t(B) * kLbDesc);
+  std::vector<std::pair<std::pair<int, int>, long long>> placed;   // (in, out) -> element offset
+  std::vector<PackedTable> order;
+  long long n_tab = 0, tmp_bytes = 0, src_bytes = 0;
+  auto place = [&](int in, int out, long long* off, long long* ks) {
+    for (size_t j = 0; j < placed.size(); ++j)
+      if (placed[j].first == std::make_pair(in, out)) { *off = placed[j].second; *ks = order[j].ksize; return; }
+    PackedTable t = lb_table(in, out);
+    placed.emplace_back(std::make_pair(in, out), n_tab);
+    *off = n_tab;
+    *ks = t.ksize;
+    n_tab += (long long)t.data.size();
+    order.push_back(std::move(t));
+  };
+  for (int b = 0; b < B; ++b) {
+    const int* g = geom_host + 6LL * b;
+    const int H = g[0], W = g[1], Wr = g[2], Hr = g[3];
+    long long* d = desc.data() + size_t(b) * kLbDesc;
+    d[kLbSrc] = src_bytes;
+    src_bytes += 3LL * H * W;
+    d[kLbH] = H; d[kLbW] = W; d[kLbWr] = Wr; d[kLbHr] = Hr; d[kLbPadL] = g[4]; d[kLbPadT] = g[5];
+    d[kLbTmp] = d[kLbHTab] = d[kLbHK] = d[kLbVTab] = d[kLbVK] = -1;
+    if (Wr != W) {   // Pillow skips a pass whose size does not change
+      d[kLbTmp] = tmp_bytes;
+      tmp_bytes += 3LL * H * Wr;
+      place(W, Wr, &d[kLbHTab], &d[kLbHK]);
+    }
+    if (Hr != H) place(H, Hr, &d[kLbVTab], &d[kLbVK]);
+  }
+  if (tables_host && tables_capacity < n_tab) return set_error("letterbox_batch_plan: the table buffer is too small");
+  sizes_host[0] = n_tab; sizes_host[1] = tmp_bytes; sizes_host[2] = src_bytes;
+  if (!tables_host) return 0;
+  memcpy(desc_host, desc.data(), desc.size() * sizeof(long long));
+  for (size_t j = 0; j < order.size(); ++j)
+    memcpy(tables_host + placed[j].second, order[j].data.data(), order[j].data.size() * sizeof(int));
+  return 0;
+}
+
+// src / tmp: flat device buffers addressed by the descriptors' byte offsets; canvas: device u8 [B][Th][Tw][3].
+int b2p_letterbox_batch(const unsigned char* src, int B, const long long* desc_host, const long long* desc, const int* tables,
+                        int Tw, int Th, unsigned char* tmp, unsigned char* canvas, cudaStream_t st) {
+  if (B < 1 || B > 65535) return set_error("letterbox_batch: B must be in [1, 65535]");
+  if (Tw < 1 || Th < 1) return set_error("letterbox_batch: the canvas must be at least 1 x 1");
+  long long h_max = 0;
+  for (int b = 0; b < B; ++b) {
+    const long long* d = desc_host + (long long)b * kLbDesc;
+    if (int e = lb_check_geometry(d[kLbH], d[kLbW], d[kLbWr], d[kLbHr], d[kLbPadL], d[kLbPadT], Tw, Th, "letterbox_batch"))
+      return e;
+    const bool h = d[kLbWr] != d[kLbW], v = d[kLbHr] != d[kLbH];
+    if (d[kLbSrc] < 0 || h != (d[kLbHTab] >= 0) || v != (d[kLbVTab] >= 0) || (h && (d[kLbHK] < 1 || d[kLbTmp] < 0)) ||
+        (v && d[kLbVK] < 1))
+      return set_error("letterbox_batch: a descriptor's offsets or tables disagree with its geometry");
+    if (h) h_max = std::max(h_max, d[kLbH] * d[kLbWr]);
+  }
+  const long long cap = std::max(1LL, (132LL * 16 + B - 1) / B);   // grid_for's cap, shared by the images
+  if (h_max) {
+    lanczos_h_batch_kernel<<<dim3(unsigned(std::min(cap, (h_max + 255) / 256)), B), 256, 0, st>>>(src, desc, tables, tmp);
+    B2P_CHECK_LAUNCH();
+  }
+  const long long v_chunks = std::min(cap, ((long long)Tw * Th + 255) / 256);
+  launch_pdl(lanczos_v_paste_batch_kernel, dim3(unsigned(v_chunks), B), dim3(256), 0, st, src, desc, tables,
+             (const unsigned char*)tmp, Tw, Th, canvas);
   B2P_CHECK_LAUNCH();
   return 0;
 }

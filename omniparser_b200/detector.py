@@ -29,16 +29,20 @@ class Result:  # ref:util/yolov9.py:22-24
         self.boxes = boxes
 
 
-def _geometry(w: int, h: int, imgsz):
-    """ref:util/yolov9.py:52-61,73-80."""
+def _canvas(imgsz):
+    """(tw, th) of the letterbox canvas, ref:util/yolov9.py:52-61."""
     if isinstance(imgsz, int):
         tw = th = imgsz
     elif len(imgsz) == 2:
         th, tw = imgsz
     else:
         raise ValueError(f"Expected one or two image dimensions, got {imgsz}")
-    tw = ((int(tw) + 31) // 32) * 32
-    th = ((int(th) + 31) // 32) * 32
+    return ((int(tw) + 31) // 32) * 32, ((int(th) + 31) // 32) * 32
+
+
+def _geometry(w: int, h: int, imgsz):
+    """ref:util/yolov9.py:52-61,73-80."""
+    tw, th = _canvas(imgsz)
     scale = min(tw / w, th / h)
     rw, rh = int(w * scale), int(h * scale)
     if rw < 1 or rh < 1:   # Pillow's resize raises the same (e.g. 641 x 1 at imgsz 640 resizes to 640 x 0)
@@ -99,63 +103,189 @@ class B200YOLOv9Detector:
         with Image.open(source) as im:
             return np.asarray(im.convert("RGB"))
 
+    def _common_io(self, B, th, tw, max_det):
+        """The buffers of an io slot that do not depend on the screenshots' size: detector plan of (B, th, tw), candidates,
+        NMS outputs and the device overlap filter's buffers."""
+        dev = self.device
+        pk = (B, th, tw)
+        if pk not in self._plans:
+            self._plans[pk] = YoloPlan(self.weights, B, th, tw, self.use_graph)
+        plan = self._plans[pk]
+        A = sum(h * w for h, w in plan.hw)
+        cap = min(self.CAND_CAP, A)
+        f32 = dict(dtype=torch.float32, device=dev)
+        io = dict(
+            plan=plan, cap=cap,
+            host_count=torch.zeros((B,), dtype=torch.int32).pin_memory(),
+            host_box=torch.zeros((B, max_det, 4), dtype=torch.float32).pin_memory(),
+            host_cand=torch.zeros((B,), dtype=torch.int32).pin_memory(),
+            cand_box=torch.empty((B, cap, 4), **f32), cand_score=torch.empty((B, cap), **f32),
+            cand_cls=torch.empty((B, cap), dtype=torch.int32, device=dev),
+            cand_count=torch.zeros((B,), dtype=torch.int32, device=dev),
+            keep=torch.empty((B, max_det), dtype=torch.int32, device=dev),
+            out_box=torch.empty((B, max_det, 4), **f32), out_score=torch.empty((B, max_det), **f32),
+            out_count=torch.zeros((B,), dtype=torch.int32, device=dev),
+        )
+        # device overlap filter (b2p_overlap_filter, ref:util/utils.py:241-319): OCR ratio boxes in, flags + crop list out
+        mo = self.OCR_CAP
+        i32 = dict(dtype=torch.int32, device=dev)
+        io.update(
+            max_ocr=mo,
+            ocr_ratio=torch.zeros((B, mo, 4), **f32), ocr_count=torch.zeros((B,), **i32),
+            host_ocr_ratio=torch.zeros((B, mo, 4), dtype=torch.float32).pin_memory(),
+            host_ocr_count=torch.zeros((B,), dtype=torch.int32).pin_memory(),
+            icon_state=torch.zeros((B, max_det), **i32), label_mask=torch.zeros((B, max_det, mo // 32), **i32),
+            ocr_removed=torch.zeros((B, mo), **i32), icon_ratio=torch.zeros((B, max_det, 4), **f32),
+            crop_box=torch.zeros((B * max_det, 4), **f32), crop_img=torch.zeros((B * max_det,), **i32),
+            crop_counts=torch.zeros((B + 1,), **i32), arrive=torch.zeros((1,), **i32),
+            host_state=torch.zeros((B, max_det), dtype=torch.int32).pin_memory(),
+            host_mask=torch.zeros((B, max_det, mo // 32), dtype=torch.int32).pin_memory(),
+            host_removed=torch.zeros((B, mo), dtype=torch.int32).pin_memory(),
+            host_ratio=torch.zeros((B, max_det, 4), dtype=torch.float32).pin_memory(),
+            host_crop_counts=torch.zeros((B + 1,), dtype=torch.int32).pin_memory(),
+        )
+        return io
+
     def _get_io(self, B, H, W, imgsz, max_det, slot=0):
         tw, th, scale, rw, rh, pl, pt = _geometry(W, H, imgsz)
         key = (B, H, W, tw, th, max_det, slot)
         io = self._io.get(key)
         if io is None:
             dev = self.device
-            pk = (B, th, tw)
-            if pk not in self._plans:
-                self._plans[pk] = YoloPlan(self.weights, B, th, tw, self.use_graph)
-            plan = self._plans[pk]
-            A = sum(h * w for h, w in plan.hw)
-            cap = min(self.CAND_CAP, A)
             f32 = dict(dtype=torch.float32, device=dev)
-            io = dict(
-                plan=plan, geom=(tw, th, scale, rw, rh, pl, pt), cap=cap,
+            io = self._common_io(B, th, tw, max_det)
+            io.update(
+                geom=(tw, th, scale, rw, rh, pl, pt),
                 host=torch.empty((B, H, W, 3), dtype=torch.uint8).pin_memory(),
-                host_count=torch.zeros((B,), dtype=torch.int32).pin_memory(),
-                host_box=torch.zeros((B, max_det, 4), dtype=torch.float32).pin_memory(),
-                host_cand=torch.zeros((B,), dtype=torch.int32).pin_memory(),
                 src=torch.empty((B, H, W, 3), dtype=torch.uint8, device=dev),
                 tmp=torch.empty((B, H, max(rw, 1), 3), dtype=torch.uint8, device=dev),
                 pad_l=torch.full((B,), float(pl), **f32), pad_t=torch.full((B,), float(pt), **f32),
                 scale=torch.full((B,), float(np.float32(scale)), **f32),
                 img_w=torch.full((B,), float(W), **f32), img_h=torch.full((B,), float(H), **f32),
-                cand_box=torch.empty((B, cap, 4), **f32), cand_score=torch.empty((B, cap), **f32),
-                cand_cls=torch.empty((B, cap), dtype=torch.int32, device=dev),
-                cand_count=torch.zeros((B,), dtype=torch.int32, device=dev),
-                keep=torch.empty((B, max_det), dtype=torch.int32, device=dev),
-                out_box=torch.empty((B, max_det, 4), **f32), out_score=torch.empty((B, max_det), **f32),
-                out_count=torch.zeros((B,), dtype=torch.int32, device=dev),
-            )
-            # device overlap filter (b2p_overlap_filter, ref:util/utils.py:241-319): OCR ratio boxes in, flags + crop list out
-            mo = self.OCR_CAP
-            i32 = dict(dtype=torch.int32, device=dev)
-            io.update(
-                max_ocr=mo,
-                ocr_ratio=torch.zeros((B, mo, 4), **f32), ocr_count=torch.zeros((B,), **i32),
-                host_ocr_ratio=torch.zeros((B, mo, 4), dtype=torch.float32).pin_memory(),
-                host_ocr_count=torch.zeros((B,), dtype=torch.int32).pin_memory(),
-                icon_state=torch.zeros((B, max_det), **i32), label_mask=torch.zeros((B, max_det, mo // 32), **i32),
-                ocr_removed=torch.zeros((B, mo), **i32), icon_ratio=torch.zeros((B, max_det, 4), **f32),
-                crop_box=torch.zeros((B * max_det, 4), **f32), crop_img=torch.zeros((B * max_det,), **i32),
-                crop_counts=torch.zeros((B + 1,), **i32), arrive=torch.zeros((1,), **i32),
-                host_state=torch.zeros((B, max_det), dtype=torch.int32).pin_memory(),
-                host_mask=torch.zeros((B, max_det, mo // 32), dtype=torch.int32).pin_memory(),
-                host_removed=torch.zeros((B, mo), dtype=torch.int32).pin_memory(),
-                host_ratio=torch.zeros((B, max_det, 4), dtype=torch.float32).pin_memory(),
-                host_crop_counts=torch.zeros((B + 1,), dtype=torch.int32).pin_memory(),
             )
             self._io[key] = io
         return io
+
+    # ---- screenshots of different sizes in one batch (one canvas, ragged source buffer) ----
+    @staticmethod
+    def is_mixed(images) -> bool:
+        """True for a list of screenshots that do not all have one size (a tensor batch has one size by construction)."""
+        return isinstance(images, (list, tuple)) and len({tuple(np.shape(im)[:2]) for im in images}) > 1
+
+    @staticmethod
+    def plan_mixed(sizes, imgsz):
+        """Host only: (H, W) per screenshot -> dict(canvas, geom, desc, tables, need) of one ragged batch; ``need`` = (src
+        bytes, tmp bytes, table ints) the io slot must hold."""
+        canvas, geom = None, []
+        for H, W in sizes:
+            tw, th, scale, rw, rh, pl, pt = _geometry(W, H, imgsz)
+            assert canvas in (None, (tw, th))
+            canvas = (tw, th)
+            geom.append((H, W, rw, rh, pl, pt, float(np.float32(scale))))
+        desc, tables, tmp_b, src_b = ops.letterbox_batch_plan([g[:6] for g in geom], *canvas)
+        return dict(canvas=canvas, geom=geom, desc=desc, tables=tables, need=(src_b, tmp_b, int(tables.size)))
+
+    def _get_io_mixed(self, B, imgsz, max_det, slot=0):
+        """io slot of ragged batches: keyed by the canvas, not by the screenshots' size, so batches of any composition share
+        it.  Same keys as :meth:`_get_io` (so filter_device / elements_from_io / check_capacity work unchanged), except that
+        src / tmp are flat byte buffers addressed by per-image descriptors, the per-image geometry is filled per batch, and
+        the crop metadata (meta_hw / meta_off) lives here.  Buffers are sized by :meth:`reserve_mixed`."""
+        tw, th = _canvas(imgsz)
+        key = ("mixed", B, tw, th, max_det, slot)
+        io = self._io.get(key)
+        if io is None:
+            io = self._common_io(B, th, tw, max_det)
+            io.update(mixed=True, canvas=(tw, th), B=B, cap_src=0, cap_tmp=0, cap_tab=0, src=None)
+            self._io[key] = io
+        return io
+
+    @staticmethod
+    def mixed_grow_needed(io, mb) -> bool:
+        """True when the slot already holds buffers and the batch does not fit them: growing frees buffers another stream
+        may still read, so the caller drains its pipeline first (:meth:`reserve_mixed` then synchronises)."""
+        return io["src"] is not None and not B200YOLOv9Detector._mixed_fits(io, mb["need"])
+
+    @staticmethod
+    def _mixed_fits(io, need):
+        return need[0] <= io["cap_src"] and need[1] <= io["cap_tmp"] and need[2] <= io["cap_tab"]
+
+    def reserve_mixed(self, io, mb):
+        """Size the slot's buffers for the batch.  A slot that already has buffers grows geometrically (x1.5) and only
+        after a device synchronise; steady state allocates nothing."""
+        need = mb["need"]
+        if io["src"] is not None and self._mixed_fits(io, need):
+            return
+        if io["src"] is not None:
+            torch.cuda.synchronize(self.device)
+            grow = lambda n, c: max(n, c + c // 2)                     # noqa: E731
+            need = (grow(need[0], io["cap_src"]), grow(need[1], io["cap_tmp"]), grow(need[2], io["cap_tab"]))
+        B, dev = io["B"], self.device
+        cap_src, cap_tmp, cap_tab = need
+        # the batch's small data, one H2D copy: desc int64 [B,12] | meta_off int64 [B] | pad_l, pad_t, scale, img_w, img_h
+        # f32 [B] | meta_hw int32 [B,2] | tables int32 [cap_tab]
+        o_off, o_f32 = B * ops.LB_DESC * 8, B * (ops.LB_DESC + 1) * 8
+        o_hw = o_f32 + 5 * B * 4
+        o_tab = (o_hw + 8 * B + 15) // 16 * 16
+        small_bytes = o_tab + 4 * max(cap_tab, 1)
+        host_small = torch.zeros((small_bytes,), dtype=torch.uint8).pin_memory()
+        small = torch.zeros((small_bytes,), dtype=torch.uint8, device=dev)
+
+        def views(buf):
+            f = buf[o_f32:o_hw].view(torch.float32)
+            return dict(desc=buf[:o_off].view(torch.int64).view(B, ops.LB_DESC), meta_off=buf[o_off:o_f32].view(torch.int64),
+                        pad_l=f[:B], pad_t=f[B:2 * B], scale=f[2 * B:3 * B], img_w=f[3 * B:4 * B], img_h=f[4 * B:],
+                        meta_hw=buf[o_hw:o_hw + 8 * B].view(torch.int32).view(B, 2), tables=buf[o_tab:].view(torch.int32))
+        io.update(views(small))
+        io.update(small=small, host_small=host_small, host_views=views(host_small), small_layout=o_tab,
+                  host=torch.empty((max(cap_src, 1),), dtype=torch.uint8).pin_memory(),
+                  src=torch.empty((max(cap_src, 1),), dtype=torch.uint8, device=dev),
+                  tmp=torch.empty((max(cap_tmp, 1),), dtype=torch.uint8, device=dev),
+                  cap_src=cap_src, cap_tmp=cap_tmp, cap_tab=cap_tab)
+
+    def stage_mixed(self, io, mb, images):
+        """Pack the screenshots and the batch's small data into the slot's pinned buffers and copy both to the device on the
+        current stream (two H2D copies).  The slot must hold the batch (:meth:`reserve_mixed`)."""
+        assert self._mixed_fits(io, mb["need"]) and len(images) == io["B"] == len(mb["geom"])
+        B = io["B"]
+        hv, host = io["host_views"], io["host"]
+        hv["desc"].numpy()[:] = mb["desc"]
+        g = np.asarray(mb["geom"], dtype=np.float64)
+        hv["meta_off"].numpy()[:] = mb["desc"][:, 0]
+        for name, col in (("pad_l", 4), ("pad_t", 5), ("scale", 6), ("img_w", 1), ("img_h", 0)):
+            hv[name].numpy()[:] = g[:, col].astype(np.float32)
+        hv["meta_hw"].numpy()[:] = g[:, :2].astype(np.int32)
+        n_tab = mb["need"][2]
+        hv["tables"].numpy()[:n_tab] = mb["tables"]
+        hn = host.numpy()
+        for i, im in enumerate(images):
+            H, W = mb["geom"][i][:2]
+            assert im.shape == (H, W, 3) and im.dtype == np.uint8
+            o = int(mb["desc"][i, 0])
+            hn[o:o + 3 * H * W] = np.ascontiguousarray(im).reshape(-1)
+        n_small = io["small_layout"] + 4 * n_tab
+        io["small"][:n_small].copy_(io["host_small"][:n_small], non_blocking=True)
+        n_src = mb["need"][0]
+        io["src"][:n_src].copy_(host[:n_src], non_blocking=True)
+        io["sizes"] = [tuple(x[:2]) for x in mb["geom"]]
+
+    def detect_device_mixed(self, io, sizes, conf, iou, max_det):
+        """After :meth:`stage_mixed`, on the same stream: ragged letterbox -> forward -> decode -> NMS (no host sync)."""
+        assert [tuple(s) for s in sizes] == io["sizes"]
+        plan: YoloPlan = io["plan"]
+        tw, th = io["canvas"]
+        ops.letterbox_batch(io["src"], len(sizes), io["host_views"]["desc"], io["desc"], io["tables"], tw, th, io["tmp"],
+                            plan.canvas)
+        self._forward_nms(io, len(sizes), conf, iou, max_det)
 
     def detect_device(self, io, B, H, W, conf, iou, max_det):
         """Device-resident u8 images in io['src'] -> NMS outputs in io (no host sync)."""
         plan: YoloPlan = io["plan"]
         tw, th, scale, rw, rh, pl, pt = io["geom"]
         ops.letterbox(io["src"], B, H, W, rw, rh, tw, th, pl, pt, io["tmp"], plan.canvas)
+        self._forward_nms(io, B, conf, iou, max_det)
+
+    def _forward_nms(self, io, B, conf, iou, max_det):
+        plan: YoloPlan = io["plan"]
         plan.run()
         ops.yolo_decode(plan.cls_out, plan.box_out, plan.hw, self.weights.nc, B, float(conf), io["pad_l"], io["pad_t"],
                         io["scale"], io["cap"], io["cand_box"], io["cand_score"], io["cand_cls"], io["cand_count"])
@@ -205,8 +335,17 @@ class B200YOLOv9Detector:
 
     @torch.inference_mode()
     def predict_batch(self, images: Sequence[np.ndarray], conf=0.25, imgsz=640, iou=0.7, max_det=300) -> List[Result]:
-        """Same-size u8 HWC images -> one Result per image (one H2D copy, one D2H of the counts)."""
+        """u8 HWC images -> one Result per image (one H2D copy of the screenshots, one D2H of the counts).  Screenshots of
+        different sizes share one batch through the ragged letterbox; same-size ones take the one-size path."""
         B = len(images)
+        if self.is_mixed(list(images)):
+            with self._lock, torch.cuda.device(self.device):
+                mb = self.plan_mixed([im.shape[:2] for im in images], imgsz)
+                io = self._get_io_mixed(B, imgsz, max_det)
+                self.reserve_mixed(io, mb)
+                self.stage_mixed(io, mb, images)
+                self.detect_device_mixed(io, [im.shape[:2] for im in images], conf, iou, max_det)
+                return self._results(io)
         H, W = images[0].shape[:2]
         with self._lock, torch.cuda.device(self.device):
             io = self._get_io(B, H, W, imgsz, max_det)
@@ -215,9 +354,12 @@ class B200YOLOv9Detector:
                 io["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
             io["src"].copy_(io["host"], non_blocking=True)
             self.detect_device(io, B, H, W, conf, iou, max_det)
-            counts = io["out_count"].cpu().tolist()
-            self.check_capacity(io["cand_count"].cpu(), io["cap"])
-            return [Result(Boxes(io["out_box"][i, :n].clone(), io["out_score"][i, :n].clone())) for i, n in enumerate(counts)]
+            return self._results(io)
+
+    def _results(self, io):
+        counts = io["out_count"].cpu().tolist()
+        self.check_capacity(io["cand_count"].cpu(), io["cap"])
+        return [Result(Boxes(io["out_box"][i, :n].clone(), io["out_score"][i, :n].clone())) for i, n in enumerate(counts)]
 
     @torch.inference_mode()
     def predict(self, source, conf=0.25, imgsz=640, iou=0.7, max_det=300):

@@ -244,6 +244,33 @@ def letterbox(src_u8, B, H, W, Wr, Hr, Tw, Th, pad_l, pad_t, tmp, canvas):
                                         _stream()))
 
 
+LB_DESC = 12   # int64 fields per image of a ragged letterbox descriptor (include/b200parse.h)
+
+
+def letterbox_batch_plan(geom, Tw, Th):
+    """Host only.  geom: per image (H, W, Wr, Hr, pad_l, pad_t) -> (desc int64 [B, 12], tables int32 [n], tmp bytes, src
+    bytes) of :func:`letterbox_batch` (b2p_letterbox_batch_plan_host)."""
+    import numpy as np
+    g = np.ascontiguousarray(np.asarray(geom, dtype=np.int32).reshape(-1, 6))
+    B = g.shape[0]
+    sizes = np.zeros(3, np.int64)
+    lib = _lib.lib()
+    _lib.check(lib.b2p_letterbox_batch_plan_host(B, g.ctypes.data, Tw, Th, None, None, 0, sizes.ctypes.data))
+    desc = np.zeros((B, LB_DESC), np.int64)
+    tables = np.zeros(max(int(sizes[0]), 1), np.int32)
+    _lib.check(lib.b2p_letterbox_batch_plan_host(B, g.ctypes.data, Tw, Th, desc.ctypes.data, tables.ctypes.data,
+                                                 tables.size, sizes.ctypes.data))
+    return desc, tables[:int(sizes[0])], int(sizes[1]), int(sizes[2])
+
+
+def letterbox_batch(src_u8, B, desc_host, desc, tables, Tw, Th, tmp, canvas):
+    """Screenshots of different sizes (flat ``src_u8``, per-image descriptors from :func:`letterbox_batch_plan`) -> canvas
+    [B, Th, Tw, 3].  ``desc_host``: the descriptors in host memory (CPU tensor or numpy); ``desc`` / ``tables``: device copies."""
+    hp = desc_host.ctypes.data if hasattr(desc_host, "ctypes") else desc_host.data_ptr()
+    _lib.check(_lib.lib().b2p_letterbox_batch(_p(src_u8), B, C.c_void_p(hp), _p(desc), _p(tables), Tw, Th, _p(tmp),
+                                              _p(canvas), _stream()))
+
+
 def resize_u8(src_u8, B, H, W, Wr, Hr, filt, tmp, out):
     """Pillow-exact resize; filt 0 = LANCZOS, 1 = BICUBIC."""
     _lib.check(_lib.lib().b2p_resize_u8(_p(src_u8), B, H, W, Wr, Hr, filt, _p(tmp), _p(out), _stream()))

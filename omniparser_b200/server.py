@@ -5,8 +5,8 @@ time: ``Omniparser.parse(base64_image)`` -> ``{"som_image_base64", "parsed_conte
 batch of 8 screenshots costs far less than 8 times one screenshot, so the throughput of a serving process is decided by
 whether concurrent requests share a batch.  :class:`BatchingOmniparser` keeps the facade's interface (``parse(base64) ->
 (png_b64, parsed_content_list)``, same config keys) and is safe to call from any number of threads: requests that arrive
-within ``max_wait_ms`` of each other and have the same image size are parsed in ONE ``parse_screenshots`` call (one H2D copy,
-one detector forward, one Florence-2 pass); PNG decode, the OCR pre-step, the overlay drawing and the PNG encode run on the
+within ``max_wait_ms`` of each other are parsed in ONE ``parse_screenshots`` call whatever their image sizes (they share
+the detector's 640 x 640 canvas: one detector forward, one Florence-2 pass); PNG decode, the OCR pre-step, the overlay drawing and the PNG encode run on the
 callers' own threads, outside the batch.  ``create_app`` builds the FastAPI application with the reference's routes and wire
 format (base64 PNG in JSON both ways, ref:omnitool/gradio/agent/llm_utils/omniparserclient.py:17-23).
 
@@ -152,7 +152,9 @@ class BatchingOmniparser:
         img = np.asarray(image.convert("RGB"))
         if not ocr_bbox:
             print("no ocr bbox!!!")
-        elems = self._batcher.submit(img.shape[:2], dict(img=img, text=list(text), ocr_bbox=ocr_bbox or None))
+        # queued by detector canvas: every request through this facade letterboxes to 640 x 640, so screenshots of any size
+        # share a batch (parse_screenshots takes a batch of different sizes)
+        elems = self._batcher.submit((640, 640), dict(img=img, text=list(text), ocr_bbox=ocr_bbox or None))
         print("len(filtered_boxes):", len(elems), -1)
         encoded, _, _ = som_overlay.som_outputs(img, [e["bbox"] for e in elems], True, **cfg)
         return encoded, elems

@@ -88,6 +88,21 @@ def _check_crop_status(status: torch.Tensor) -> None:
         raise RuntimeError(f"{bad} crop boxes were empty after truncation (status flags of b2p_crop_resize)")
 
 
+def _crop_meta(model: B200YOLOv9Detector, io_, B, H, W, *key):
+    """(img_hw, img_off) of b2p_crop_resize for a batch's screenshots in io_["src"]: a ragged batch's are filled per batch in
+    its io slot; a one-size batch's are built once per (B, H, W, *key) and cached on the detector handle."""
+    if io_.get("mixed"):
+        return io_["meta_hw"], io_["meta_off"]
+    key = ("crop_meta", B, H, W) + key
+    meta = model._io.get(key)
+    if meta is None:
+        dev = model.device
+        meta = dict(hw=torch.tensor([[H, W]] * B, dtype=torch.int32, device=dev),
+                    off=torch.tensor([i * H * W * 3 for i in range(B)], dtype=torch.int64, device=dev))
+        model._io[key] = meta
+    return meta["hw"], meta["off"]
+
+
 @torch.inference_mode()
 def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, caption_model_processor: dict,
                       ocr: Sequence[tuple], BOX_TRESHOLD=0.01, iou_threshold=0.9, imgsz=640, max_new_tokens=20,
@@ -96,7 +111,8 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
                       early_stopping=None, length_penalty=None):
     """``caption_size`` 64 = the reference's CUDA branch (crops captioned at 64x64, ref:util/utils.py:121); 768 = its
     CPU branch (CLIP processor bicubic-resizes every crop to 768x768 first, :123), done on the device, in chunks.
-    Same-size u8 HWC screenshots + per-image ``(ocr_text, ocr_bbox_xyxy_pixels)`` -> per-image
+    u8 HWC screenshots (of one size, or of different sizes: those share one detector batch through the ragged letterbox)
+    + per-image ``(ocr_text, ocr_bbox_xyxy_pixels)`` -> per-image
     ``(filtered_boxes_elem, caption_token_ids)``; the compute of ``get_som_labeled_img`` without the overlay drawing.
     NMS IoU is fixed at 0.1 as in ref:util/utils.py:431; ``iou_threshold`` feeds the overlap filter (:446).
     ``num_beams`` > 1 captions with HF beam search (one caption per crop; early_stopping / length_penalty default to the
@@ -104,21 +120,35 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
     bs = beam_settings(num_beams, False, early_stopping, length_penalty, 1, caption_model_processor["model"].beam_defaults)
     bs.pop("num_return_sequences")
     B = len(images)
-    H, W = images[0].shape[:2]
+    mixed = B200YOLOv9Detector.is_mixed(images)
+    if mixed and _skip_h2d:
+        raise ValueError("_skip_h2d takes screenshots of one size: a batch of different sizes has no resident one-size buffer")
+    H, W = (None, None) if mixed else images[0].shape[:2]
+    sizes = [tuple(im.shape[:2]) for im in images] if mixed else [(H, W)] * B
     cap_model: B200Florence2Model = caption_model_processor["model"]
     processor = caption_model_processor["processor"]
     t0 = time.perf_counter()
     with model._lock, torch.cuda.device(model.device):   # io slot 0 / caption plan instance 0 are this handle's: one call at a time
-        io_ = model._get_io(B, H, W, imgsz, 300)
-        if not _skip_h2d:   # bench "value" leg: the u8 screenshots are already resident in io_["src"]
+        if mixed:
+            mb = model.plan_mixed(sizes, imgsz)
+            io_ = model._get_io_mixed(B, imgsz, 300)
+            model.reserve_mixed(io_, mb)
+            model.stage_mixed(io_, mb, images)
+        else:
+            io_ = model._get_io(B, H, W, imgsz, 300)
+        if not mixed and not _skip_h2d:   # bench "value" leg: the u8 screenshots are already resident in io_["src"]
             for i, im in enumerate(images):
                 io_["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
             io_["src"].copy_(io_["host"], non_blocking=True)
-        whwh = torch.Tensor([W, H, W, H])
-        ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / whwh).tolist() if ob else None, tx, W, H) for tx, ob in ocr]   # :437-444
+        whwh = [torch.Tensor([w, h, w, h]) for h, w in sizes]
+        ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / whwh[i]).tolist() if ob else None, tx, sizes[i][1], sizes[i][0])
+                     for i, (tx, ob) in enumerate(ocr)]   # :437-444
         on_device = False
         if _det_override is None:
-            model.detect_device(io_, B, H, W, BOX_TRESHOLD, 0.1, 300)
+            if mixed:
+                model.detect_device_mixed(io_, sizes, BOX_TRESHOLD, 0.1, 300)
+            else:
+                model.detect_device(io_, B, H, W, BOX_TRESHOLD, 0.1, 300)
             on_device = not _HOST_GLUE and model.filter_device(io_, B, H, W, ocr_elems, iou_threshold, 300)
             counts = io_["out_count"].cpu().tolist()                   # D2H #1 (sync; the filter's flags ride along)
             boxes = None if on_device else io_["out_box"].cpu()
@@ -135,10 +165,10 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
             n = int(io_["host_crop_counts"][B])
         else:
             for i in range(B):
-                xyxy = (boxes[i][:counts[i]] / whwh).tolist()              # ref:util/utils.py:432
+                xyxy = (boxes[i][:counts[i]] / whwh[i]).tolist()           # ref:util/utils.py:432
                 texts, obox = ocr[i]
-                oratio = (torch.tensor(obox) / whwh).tolist() if obox else None   # :437-442
-                elems, start = host_glue.build_elements(xyxy, oratio, texts, W, H, iou_threshold)
+                oratio = (torch.tensor(obox) / whwh[i]).tolist() if obox else None   # :437-442
+                elems, start = host_glue.build_elements(xyxy, oratio, texts, sizes[i][1], sizes[i][0], iou_threshold)
                 all_elems.append(elems)
                 for e in elems:
                     if e["content"] is None:
@@ -160,14 +190,9 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
             else:
                 d_boxes = torch.tensor(crop_boxes, dtype=torch.float32).to(dev, non_blocking=True)
                 d_bimg = torch.tensor(crop_img, dtype=torch.int32).to(dev, non_blocking=True)
-            key = ("crop_meta", B, H, W)
-            meta = model._io.get(key)
-            if meta is None:
-                meta = dict(hw=torch.tensor([[H, W]] * B, dtype=torch.int32, device=dev),
-                            off=torch.tensor([i * H * W * 3 for i in range(B)], dtype=torch.int64, device=dev))
-                model._io[key] = meta
+            hw, off = _crop_meta(model, io_, B, H, W)
             status = torch.zeros((n,), dtype=torch.int32, device=dev)
-            ops.crop_resize(io_["src"], meta["hw"], meta["off"], d_boxes, d_bimg, n, 64, crops_dst, status)
+            ops.crop_resize(io_["src"], hw, off, d_boxes, d_bimg, n, 64, crops_dst, status)
             if caption_size == 64:
                 ids = cap_model.generate_from_device_crops(plan, n).cpu()  # D2H #2 (sync)
             else:
@@ -199,7 +224,7 @@ class _Member:
 
 
 class PipelinedParser:
-    """Three-stage software pipeline over batches of same-size screenshots: detection of batch i+1 (stream A), the host
+    """Three-stage software pipeline over batches of screenshots: detection of batch i+1 (stream A), the host
     list logic of batch i and the captioning of batch i-1 (stream B) run concurrently.  Same results as :func:`parse_screenshots`, batch by
     batch; only the scheduling differs.  Usage::
 
@@ -235,29 +260,44 @@ class PipelinedParser:
         self.group = max(1, int(caption_group))
 
     @torch.inference_mode()
-    def _submit(self, slot: int, images, resident_src=None, ocr=None):
+    def _submit(self, slot: int, images, resident_src=None, ocr=None, mb=None):
         torch.cuda.set_device(self.model.device)   # runs on the worker thread: device and inference mode are thread-local
         B = len(images)
-        H, W = images[0].shape[:2]
         m = self.model
-        io_ = m._get_io(B, H, W, self.imgsz, 300, slot)
-        with torch.cuda.stream(self.s_det):
+        if mb is not None:   # screenshots of different sizes (run() has sized the slot: see _ensure_io)
             if resident_src is not None:
-                io_["src"].copy_(resident_src, non_blocking=True)
-            elif torch.is_tensor(images) and images.is_pinned():
-                # caller-owned page-locked [B,H,W,3] u8 batch: DMA straight from it (it must stay untouched until the
-                # batch's result has been yielded); pageable numpy screenshots go through the slot's pinned staging copy
-                io_["src"].copy_(images, non_blocking=True)
+                raise ValueError("resident= batches have one size: a batch of different sizes has no one-size device tensor")
+            sizes = [tuple(im.shape[:2]) for im in images]
+            H = W = None
+            io_ = m._get_io_mixed(B, self.imgsz, 300, slot)
+            assert not m.mixed_grow_needed(io_, mb)
+            m.reserve_mixed(io_, mb)
+        else:
+            H, W = images[0].shape[:2]
+            sizes = [(H, W)] * B
+            io_ = m._get_io(B, H, W, self.imgsz, 300, slot)
+        with torch.cuda.stream(self.s_det):
+            if mb is not None:
+                m.stage_mixed(io_, mb, images)
+                m.detect_device_mixed(io_, sizes, self.conf, 0.1, 300)
             else:
-                for i, im in enumerate(images):
-                    io_["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
-                io_["src"].copy_(io_["host"], non_blocking=True)
-            m.detect_device(io_, B, H, W, self.conf, 0.1, 300)
+                if resident_src is not None:
+                    io_["src"].copy_(resident_src, non_blocking=True)
+                elif torch.is_tensor(images) and images.is_pinned():
+                    # caller-owned page-locked [B,H,W,3] u8 batch: DMA straight from it (it must stay untouched until the
+                    # batch's result has been yielded); pageable numpy screenshots go through the slot's pinned staging copy
+                    io_["src"].copy_(images, non_blocking=True)
+                else:
+                    for i, im in enumerate(images):
+                        io_["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
+                    io_["src"].copy_(io_["host"], non_blocking=True)
+                m.detect_device(io_, B, H, W, self.conf, 0.1, 300)
             ocr_elems, on_device = None, False
             if ocr is not None and not _HOST_GLUE:
                 # overlap filter on the device, right behind NMS on the detector's stream (no host round trip in between)
-                whwh = torch.Tensor([W, H, W, H])
-                ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / whwh).tolist() if ob else None, tx, W, H) for tx, ob in ocr]
+                whwh = [torch.Tensor([w, h, w, h]) for h, w in sizes]
+                ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / whwh[i]).tolist() if ob else None, tx, sizes[i][1], sizes[i][0])
+                             for i, (tx, ob) in enumerate(ocr)]
                 on_device = m.filter_device(io_, B, H, W, ocr_elems, self.iou_thr, 300)
             io_["host_count"].copy_(io_["out_count"], non_blocking=True)
             if not on_device:
@@ -265,7 +305,7 @@ class PipelinedParser:
             io_["host_cand"].copy_(io_["cand_count"], non_blocking=True)
             ev = torch.cuda.Event()
             ev.record(self.s_det)
-        return dict(io=io_, ev=ev, B=B, H=H, W=W, ocr_elems=ocr_elems, on_device=on_device)
+        return dict(io=io_, ev=ev, B=B, H=H, W=W, sizes=sizes, ocr_elems=ocr_elems, on_device=on_device)
 
     def _glue(self, h, ocr):
         """Stage 2 (caller's thread): wait for the detector's boxes, run the reference's host list logic."""
@@ -283,12 +323,12 @@ class PipelinedParser:
             all_elems = None
         else:
             boxes = io_["host_box"]
-            whwh = torch.Tensor([W, H, W, H])
-            for i in range(B):
+            for i, (hi, wi) in enumerate(h["sizes"]):
+                whwh = torch.Tensor([wi, hi, wi, hi])
                 xyxy = (boxes[i][:counts[i]] / whwh).tolist()
                 texts, obox = ocr[i]
                 oratio = (torch.tensor(obox) / whwh).tolist() if obox else None
-                elems, _ = host_glue.build_elements(xyxy, oratio, texts, W, H, self.iou_thr)
+                elems, _ = host_glue.build_elements(xyxy, oratio, texts, wi, hi, self.iou_thr)
                 all_elems.append(elems)
                 for e in elems:
                     if e["content"] is None:
@@ -324,14 +364,9 @@ class PipelinedParser:
                 else:
                     d_boxes = torch.tensor(crop_boxes, dtype=torch.float32).to(dev, non_blocking=True)
                     d_bimg = torch.tensor(crop_img, dtype=torch.int32).to(dev, non_blocking=True)
-                key = ("crop_meta", B, H, W, lane)
-                meta = model._io.get(key)
-                if meta is None:
-                    meta = dict(hw=torch.tensor([[H, W]] * B, dtype=torch.int32, device=dev),
-                                off=torch.tensor([i * H * W * 3 for i in range(B)], dtype=torch.int64, device=dev))
-                    model._io[key] = meta
+                hw, off = _crop_meta(model, io_, B, H, W, lane)
                 status = torch.zeros((n,), dtype=torch.int32, device=dev)
-                ops.crop_resize(io_["src"], meta["hw"], meta["off"], d_boxes, d_bimg, n, 64, plan.crops, status)
+                ops.crop_resize(io_["src"], hw, off, d_boxes, d_bimg, n, 64, plan.crops, status)
                 ids = cap_model.generate_from_device_crops(plan, n)
                 if all_elems is None:   # device overlap filter: element lists from its flags, while the GPU captions
                     all_elems = [model.elements_from_io(io_, i, g["counts"][i], h["ocr_elems"][i]) for i in range(B)]
@@ -380,14 +415,9 @@ class PipelinedParser:
                     else:
                         d_boxes = torch.tensor(g["crop_boxes"], dtype=torch.float32).to(dev, non_blocking=True)
                         d_bimg = torch.tensor(g["crop_img"], dtype=torch.int32).to(dev, non_blocking=True)
-                    key = ("crop_meta", B, H, W, lane)
-                    meta = model._io.get(key)
-                    if meta is None:
-                        meta = dict(hw=torch.tensor([[H, W]] * B, dtype=torch.int32, device=dev),
-                                    off=torch.tensor([i * H * W * 3 for i in range(B)], dtype=torch.int64, device=dev))
-                        model._io[key] = meta
+                    hw, moff = _crop_meta(model, io_, B, H, W, lane)
                     status = torch.zeros((ng,), dtype=torch.int32, device=dev)
-                    ops.crop_resize(io_["src"], meta["hw"], meta["off"], d_boxes, d_bimg, ng, 64, plan.crops[off:], status)
+                    ops.crop_resize(io_["src"], hw, moff, d_boxes, d_bimg, ng, 64, plan.crops[off:], status)
                     off += ng
                 ids = cap_model.generate_from_device_crops(plan, n).cpu()
         t3 = time.perf_counter()
@@ -419,8 +449,8 @@ class PipelinedParser:
 
     @torch.inference_mode()
     def run(self, batches, resident=None):
-        """batches: iterable of (images, ocr), images a list of same-size u8 HWC numpy arrays or one page-locked u8 torch
-        tensor [B,H,W,3]; resident: optional parallel iterable of device u8 tensors [B,H,W,3] (skips the H2D copy).
+        """batches: iterable of (images, ocr), images a list of u8 HWC numpy arrays (of one size, or of different sizes: a
+        ragged batch, batch by batch) or one page-locked u8 torch tensor [B,H,W,3]; resident: optional parallel iterable of device u8 tensors [B,H,W,3] (skips the H2D copy).
         Stages in flight: detect(i+1) on stream A (submit thread) | host list logic of batch i (this thread) |
         caption(i-1), caption(i-2) on their lane's stream (caption threads).  lanes + 2 io slots (more with caption_group) keep a batch's resident
         screenshots alive until its crops have been cut.  Results come out in order, ``lanes`` batches behind the glue."""
@@ -433,7 +463,8 @@ class PipelinedParser:
             if cur is None:
                 return
             slot = 0
-            h = self._submit(slot, cur[0], next(rit) if rit is not None else None, cur[1])
+            mb = self._ensure_io(slot, cur[0], ())
+            h = self._submit(slot, cur[0], next(rit) if rit is not None else None, cur[1], **({} if mb is None else dict(mb=mb)))
             pending = deque()
             grp = []
             while cur is not None:
@@ -443,7 +474,9 @@ class PipelinedParser:
                     # slots alive at once: lanes*group in caption + up to group-1 glued batches waiting for their group
                     # + the batch in the host list logic + the batch in detection  (= lanes + 2 when group == 1)
                     slot = (slot + 1) % (self.lanes * self.group + self.group + 1)
-                    fut = self._pool.submit(self._submit, slot, nxt[0], next(rit) if rit is not None else None, nxt[1])
+                    mb = self._ensure_io(slot, nxt[0], pending)
+                    fut = self._pool.submit(self._submit, slot, nxt[0], next(rit) if rit is not None else None, nxt[1],
+                                            **({} if mb is None else dict(mb=mb)))
                 g = self._glue(h, cur[1])
                 if self.group == 1:
                     self._ensure_plan(g, pending, fut)
@@ -483,6 +516,22 @@ class PipelinedParser:
                     if n and not cap_model.plan_ready(n, self.T, self.prompt, instance=lane):
                         cap_model.warm_plan(n, self.T, self.prompt, instance=lane, stream=self.s_caps[lane])
             torch.cuda.synchronize()
+
+    def _ensure_io(self, slot, images, pending):
+        """A batch of screenshots of different sizes -> its letterbox plan (None for a one-size batch).  When the batch does
+        not fit the buffers its io slot already holds, the pipeline is drained (every batch in flight finished, device
+        synchronised) before the slot grows: the freed buffers may still be read by another stream until then."""
+        if not B200YOLOv9Detector.is_mixed(images):
+            return None
+        m = self.model
+        mb = m.plan_mixed([tuple(im.shape[:2]) for im in images], self.imgsz)
+        io_ = m._get_io_mixed(len(images), self.imgsz, 300, slot)
+        if m.mixed_grow_needed(io_, mb):
+            for p in pending:
+                p.result()
+            torch.cuda.synchronize()
+            m.reserve_mixed(io_, mb)
+        return mb
 
     def _ensure_plan(self, g, pending, fut):
         """First batch of a crop-count bucket on a lane: drain the pipeline and build + capture the caption plan with
