@@ -192,6 +192,19 @@ int b2p_overlap_filter(const float* box_px, const int* count, int B, int max_det
 int b2p_crop_resize(const unsigned char* imgs, const int* img_hw, const long long* img_off, const float* boxes_ratio,
                     const int* box_img, int n_box, int out_hw, unsigned char* out, int* status, b2p_stream_t stream);
 
+/* ---- PNG encode of the Set-of-Marks overlay, ref:util/utils.py:493-494 (PIL Image.save(format="PNG")), lossless ----
+ * Up filter on every row; the filtered rows in bands of whole rows (about 32 KiB each), each deflated on its own (LZ77,
+ * dynamic Huffman or stored blocks, whichever is smaller) and ended byte-aligned by a sync flush; one zlib stream in one
+ * IDAT chunk.  The bytes differ from PIL's and from som_overlay.encode_png's; the decoded pixels are the frame's.
+ * b2p_png_plan_host (host only): sizes_host [3] = band count, workspace bytes, worst-case output bytes (every band
+ *   stored).  Refused: H or W < 1, a worst-case IDAT longer than 2^31 - 1 bytes.
+ * b2p_png_encode: rgb [H][W][3] contiguous u8 -> out[0..*out_len) (out_len: a device int64), asynchronous on `stream`.
+ *   Refused before any launch: what the plan refuses, null pointers, ws_bytes or out_cap below the plan's.  Never writes
+ *   past the plan's worst case (<= out_cap). */
+int b2p_png_plan_host(int H, int W, long long* sizes_host);
+int b2p_png_encode(const unsigned char* rgb, int H, int W, void* ws, long long ws_bytes, unsigned char* out, long long out_cap,
+                   long long* out_len, b2p_stream_t stream);
+
 /* ---- Florence-2 (HF generate, ref:util/utils.py:125): non-GEMM kernels; `split` selects the fp16x3 layout ---- */
 int b2p_layernorm(const float* x, long long ldx, const float* gamma, const float* beta, float eps, int T, int C,
                   void* out16, long long ld16, float* out32, long long ld32, int split, b2p_stream_t stream);

@@ -292,6 +292,19 @@ def crop_resize(imgs, img_hw, img_off, boxes, box_img, n_box, out_hw, out, statu
                                           _p(out), _p(status), _stream()))
 
 
+def png_plan(H, W):
+    """Host only: (bands, workspace bytes, worst-case PNG bytes) of :func:`png_encode` for an H x W RGB frame."""
+    import numpy as np
+    sizes = np.zeros(3, np.int64)
+    _lib.check(_lib.lib().b2p_png_plan_host(H, W, sizes.ctypes.data))
+    return int(sizes[0]), int(sizes[1]), int(sizes[2])
+
+
+def png_encode(rgb, H, W, ws, ws_bytes, out, out_cap, out_len):
+    """rgb [H, W, 3] u8 (device) -> PNG bytes in out[0 : out_len[0]] (out_len: device int64)."""
+    _lib.check(_lib.lib().b2p_png_encode(_p(rgb), H, W, _p(ws), ws_bytes, _p(out), out_cap, _p(out_len), _stream()))
+
+
 # ------------------------------------------------------------------------------------------ Florence-2 ops
 # `split=True` writes fp16 activations in the fp16x3 operand layout [hi(C) | lo(C)] (row stride 2*C).
 def layernorm(x, gamma, beta, T, C, out16=None, out32=None, eps=1e-5, split=False):

@@ -156,7 +156,8 @@ class BatchingOmniparser:
         # share a batch (parse_screenshots takes a batch of different sizes)
         elems = self._batcher.submit((640, 640), dict(img=img, text=list(text), ocr_bbox=ocr_bbox or None))
         print("len(filtered_boxes):", len(elems), -1)
-        encoded, _, _ = som_overlay.som_outputs(img, [e["bbox"] for e in elems], True, **cfg)
+        encoded, _, _ = som_overlay.som_outputs(img, [e["bbox"] for e in elems], True, **cfg,
+                                                device=getattr(self.som_model, "device", None))
         return encoded, elems
 
 

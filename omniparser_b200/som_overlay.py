@@ -17,10 +17,13 @@ Restated so that the outputs are IDENTICAL to the reference's:
 * PNG: the reference's ``PIL.Image.save(format="PNG")`` (zlib level 6) costs 80-550 ms per screenshot and dominates
   the call once the models are fast; ``encode_png`` writes the same pixels with the Up filter and a zlib level-1 stream
   deflated in parallel row bands.  The decoded image is identical; the byte stream is not (and need not be).
+  ``DevicePngEncoder`` does the same encode on the GPU (csrc/png_encode.cu: LZ77 + dynamic Huffman per row band, with
+  checksums combined across bands); ``som_outputs(device=cuda)`` uses it, every other device the host encoder.
 """
 from __future__ import annotations
 
 import base64
+import threading
 from typing import Dict, List, Sequence, Tuple
 
 import numpy as np
@@ -175,12 +178,97 @@ def encode_png(frame_rgb: np.ndarray, level: int = 1, stripes: int = 0) -> bytes
             chunk(b"IEND", b""))
 
 
+class DevicePngEncoder:
+    """PNG encode of RGB frames on one CUDA device (b2p_png_encode), for callers on any thread.  One lock serialises the
+    encodes; they run on the encoder's own role stream.  Pinned input / output staging and the device buffers grow to
+    the largest frame seen and are kept."""
+
+    def __init__(self, device):
+        import torch
+        from . import ops
+        self.device = ops._stream_device(device)
+        self.stream = ops.role_stream("png", self.device)
+        self.lock = threading.Lock()
+        self._pin_in = self._pin_out = self._dev_in = self._dev_out = self._ws = None
+        self._dev_len = None
+        self._pin_len = self._pinned(1, torch.int64)
+
+    @staticmethod
+    def _pinned(n, dtype=None):
+        import torch
+        return torch.empty(n, dtype=dtype or torch.uint8, pin_memory=True)
+
+    def _device_buf(self, n, dtype=None):
+        import torch
+        return torch.empty(n, dtype=dtype or torch.uint8, device=self.device)
+
+    @staticmethod
+    def _grow(buf, n, alloc):
+        return buf if buf is not None and buf.numel() >= n else alloc(n)
+
+    def encode(self, frame_rgb: np.ndarray) -> bytes:
+        import torch
+        from . import ops
+        h, w, c = frame_rgb.shape
+        assert c == 3 and frame_rgb.dtype == np.uint8
+        _, ws_bytes, out_cap = ops.png_plan(h, w)
+        n_in = h * w * 3
+        with self.lock:
+            self._pin_in = self._grow(self._pin_in, n_in, self._pinned)
+            self._dev_in = self._grow(self._dev_in, n_in, self._device_buf)
+            self._ws = self._grow(self._ws, ws_bytes, self._device_buf)
+            self._pin_out = self._grow(self._pin_out, out_cap, self._pinned)
+            self._dev_out = self._grow(self._dev_out, out_cap, self._device_buf)
+            if self._dev_len is None:
+                self._dev_len = self._device_buf(1, torch.int64)
+            self._pin_in[:n_in].numpy().reshape(h, w, 3)[...] = frame_rgb
+            with torch.cuda.stream(self.stream):
+                self._dev_in[:n_in].copy_(self._pin_in[:n_in], non_blocking=True)
+                ops.png_encode(self._dev_in, h, w, self._ws, self._ws.numel(), self._dev_out, self._dev_out.numel(),
+                               self._dev_len)
+                self._pin_len.copy_(self._dev_len, non_blocking=True)
+                self.stream.synchronize()
+                n = int(self._pin_len[0])
+                assert 0 < n <= out_cap, (n, out_cap)
+                self._pin_out[:n].copy_(self._dev_out[:n], non_blocking=True)
+                self.stream.synchronize()
+            return self._pin_out[:n].numpy().tobytes()
+
+
+_ENCODERS = {}
+_ENCODERS_LOCK = threading.Lock()
+
+
+def device_encoder(device) -> DevicePngEncoder:
+    """the process's encoder for ``device`` (created on first use)"""
+    from . import ops
+    key = str(ops._stream_device(device))
+    with _ENCODERS_LOCK:
+        enc = _ENCODERS.get(key)
+        if enc is None:
+            enc = _ENCODERS[key] = DevicePngEncoder(device)
+        return enc
+
+
+def _is_cuda(device) -> bool:
+    if device is None:
+        return False
+    try:
+        import torch
+        return torch.device(device).type == "cuda"
+    except (TypeError, RuntimeError):
+        return False
+
+
 def som_outputs(image_rgb: np.ndarray, boxes_xyxy_ratio: List[List[float]], output_coord_in_ratio: bool, text_scale=0.4,
-                text_padding=5, text_thickness=2, thickness=3, png_level: int = 1):
-    """Everything after the captions: -> (base64 PNG, label_coordinates) (ref:util/utils.py:478-494)."""
+                text_padding=5, text_thickness=2, thickness=3, png_level: int = 1, device=None):
+    """Everything after the captions: -> (base64 PNG, label_coordinates) (ref:util/utils.py:478-494).  With a CUDA
+    ``device`` the PNG is encoded there (:class:`DevicePngEncoder`); otherwise on the host (:func:`encode_png`).  The
+    decoded overlay is the same either way."""
     h, w = image_rgb.shape[:2]
     cxcywh = boxes_cxcywh_f32(boxes_xyxy_ratio)
     xyxy_px, xywh_px = pixel_boxes_f32(cxcywh, w, h)
     frame = annotate(image_rgb, xyxy_px, text_scale, text_padding, text_thickness, thickness)
-    encoded = base64.b64encode(encode_png(frame, png_level)).decode("ascii")
+    png = device_encoder(device).encode(frame) if _is_cuda(device) else encode_png(frame, png_level)
+    encoded = base64.b64encode(png).decode("ascii")
     return encoded, label_coordinates(xywh_px, w, h, output_coord_in_ratio), frame

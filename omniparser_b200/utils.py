@@ -599,5 +599,6 @@ def get_som_labeled_img(image_source: Union[str, Image.Image], model=None, BOX_T
     print("len(filtered_boxes):", len(elems), next((i for i, e in enumerate(elems) if e["content"] is None), -1))
     boxes = [e["bbox"] for e in elems]
     cfg = draw_bbox_config if draw_bbox_config else dict(text_scale=text_scale, text_padding=text_padding)
-    encoded, coords, _ = som_overlay.som_outputs(img, boxes, output_coord_in_ratio, **cfg)
+    encoded, coords, _ = som_overlay.som_outputs(img, boxes, output_coord_in_ratio, **cfg,
+                                                 device=getattr(model, "device", None))
     return encoded, coords, elems
