@@ -115,7 +115,7 @@ class B200YOLOv9Detector:
         cap = min(self.CAND_CAP, A)
         f32 = dict(dtype=torch.float32, device=dev)
         io = dict(
-            plan=plan, cap=cap,
+            plan=plan, cap=cap, B=B,
             host_count=torch.zeros((B,), dtype=torch.int32).pin_memory(),
             host_box=torch.zeros((B, max_det, 4), dtype=torch.float32).pin_memory(),
             host_cand=torch.zeros((B,), dtype=torch.int32).pin_memory(),
@@ -146,6 +146,18 @@ class B200YOLOv9Detector:
         )
         return io
 
+    def io_slot(self, sizes, imgsz, max_det, slot=0, drain=None):
+        """The io slot of a batch of screenshots of these (H, W) sizes, for :meth:`stage` and :meth:`detect`.  Screenshots of
+        one size get the slot of their size (:meth:`_get_io`); screenshots of different sizes share the ragged slot of their
+        canvas, which takes this batch's letterbox plan and grows when the batch does not fit its buffers.  Growing frees
+        buffers another stream may still read, so ``drain()`` (the caller finishes every batch it has in flight) runs first.
+        A slot is complete when this returns: what building or growing it launched on the caller's stream has finished, so
+        any stream may use it.  One batch owns a slot index from here until its crops have been cut."""
+        sizes = [tuple(s) for s in sizes]
+        if len(set(sizes)) > 1:
+            return self._ragged_io(sizes, imgsz, max_det, slot, drain)
+        return self._get_io(len(sizes), *sizes[0], imgsz, max_det, slot)
+
     def _get_io(self, B, H, W, imgsz, max_det, slot=0):
         tw, th, scale, rw, rh, pl, pt = _geometry(W, H, imgsz)
         key = (B, H, W, tw, th, max_det, slot)
@@ -162,47 +174,46 @@ class B200YOLOv9Detector:
                 pad_l=torch.full((B,), float(pl), **f32), pad_t=torch.full((B,), float(pt), **f32),
                 scale=torch.full((B,), float(np.float32(scale)), **f32),
                 img_w=torch.full((B,), float(W), **f32), img_h=torch.full((B,), float(H), **f32),
+                # crop metadata of b2p_crop_resize: (H, W) and byte offset of each screenshot in src
+                meta_hw=torch.tensor([[H, W]] * B, dtype=torch.int32, device=dev),
+                meta_off=torch.tensor([i * H * W * 3 for i in range(B)], dtype=torch.int64, device=dev),
             )
+            torch.cuda.synchronize(dev)   # the fills above ran on the caller's stream; other streams read the slot
             self._io[key] = io
         return io
 
     # ---- screenshots of different sizes in one batch (one canvas, ragged source buffer) ----
     @staticmethod
-    def is_mixed(images) -> bool:
-        """True for a list of screenshots that do not all have one size (a tensor batch has one size by construction)."""
-        return isinstance(images, (list, tuple)) and len({tuple(np.shape(im)[:2]) for im in images}) > 1
-
-    @staticmethod
     def plan_mixed(sizes, imgsz):
         """Host only: (H, W) per screenshot -> dict(canvas, geom, desc, tables, need) of one ragged batch; ``need`` = (src
         bytes, tmp bytes, table ints) the io slot must hold."""
-        canvas, geom = None, []
-        for H, W in sizes:
-            tw, th, scale, rw, rh, pl, pt = _geometry(W, H, imgsz)
-            assert canvas in (None, (tw, th))
-            canvas = (tw, th)
-            geom.append((H, W, rw, rh, pl, pt, float(np.float32(scale))))
-        desc, tables, tmp_b, src_b = ops.letterbox_batch_plan([g[:6] for g in geom], *canvas)
-        return dict(canvas=canvas, geom=geom, desc=desc, tables=tables, need=(src_b, tmp_b, int(tables.size)))
-
-    def _get_io_mixed(self, B, imgsz, max_det, slot=0):
-        """io slot of ragged batches: keyed by the canvas, not by the screenshots' size, so batches of any composition share
-        it.  Same keys as :meth:`_get_io` (so filter_device / elements_from_io / check_capacity work unchanged), except that
-        src / tmp are flat byte buffers addressed by per-image descriptors, the per-image geometry is filled per batch, and
-        the crop metadata (meta_hw / meta_off) lives here.  Buffers are sized by :meth:`reserve_mixed`."""
         tw, th = _canvas(imgsz)
-        key = ("mixed", B, tw, th, max_det, slot)
+        geom = []
+        for H, W in sizes:
+            _, _, scale, rw, rh, pl, pt = _geometry(W, H, imgsz)
+            geom.append((H, W, rw, rh, pl, pt, float(np.float32(scale))))
+        desc, tables, tmp_b, src_b = ops.letterbox_batch_plan([g[:6] for g in geom], tw, th)
+        return dict(canvas=(tw, th), geom=geom, desc=desc, tables=tables, need=(src_b, tmp_b, int(tables.size)))
+
+    def _ragged_io(self, sizes, imgsz, max_det, slot, drain):
+        """The ragged slot of (B, canvas, slot), sized for the batch: src / tmp are flat byte buffers addressed by per-image
+        descriptors, and the per-image geometry and crop metadata (meta_hw / meta_off) are filled per batch by :meth:`stage`
+        from ``io["batch"]``, the letterbox plan of the batch the slot was last given to."""
+        mb = self.plan_mixed(sizes, imgsz)
+        tw, th = mb["canvas"]
+        key = ("mixed", len(sizes), tw, th, max_det, slot)
         io = self._io.get(key)
         if io is None:
-            io = self._common_io(B, th, tw, max_det)
-            io.update(mixed=True, canvas=(tw, th), B=B, cap_src=0, cap_tmp=0, cap_tab=0, src=None)
-            self._io[key] = io
+            io = self._io[key] = dict(self._common_io(len(sizes), th, tw, max_det), mixed=True, canvas=(tw, th), src=None)
+        if drain is not None and self.mixed_grow_needed(io, mb):
+            drain()
+        self.reserve_mixed(io, mb)
+        io["batch"] = mb
         return io
 
     @staticmethod
     def mixed_grow_needed(io, mb) -> bool:
-        """True when the slot already holds buffers and the batch does not fit them: growing frees buffers another stream
-        may still read, so the caller drains its pipeline first (:meth:`reserve_mixed` then synchronises)."""
+        """True when the slot already holds buffers and the batch does not fit them."""
         return io["src"] is not None and not B200YOLOv9Detector._mixed_fits(io, mb["need"])
 
     @staticmethod
@@ -241,12 +252,31 @@ class B200YOLOv9Detector:
                   src=torch.empty((max(cap_src, 1),), dtype=torch.uint8, device=dev),
                   tmp=torch.empty((max(cap_tmp, 1),), dtype=torch.uint8, device=dev),
                   cap_src=cap_src, cap_tmp=cap_tmp, cap_tab=cap_tab)
+        torch.cuda.synchronize(dev)   # as in _get_io
 
-    def stage_mixed(self, io, mb, images):
-        """Pack the screenshots and the batch's small data into the slot's pinned buffers and copy both to the device on the
-        current stream (two H2D copies).  The slot must hold the batch (:meth:`reserve_mixed`)."""
-        assert self._mixed_fits(io, mb["need"]) and len(images) == io["B"] == len(mb["geom"])
-        B = io["B"]
+    def stage(self, io, images, resident=None):
+        """Copy a batch's screenshots into its io slot on the current stream: a list of u8 HWC numpy arrays through the
+        slot's pinned buffer, a page-locked [B,H,W,3] u8 tensor by DMA straight from it (the caller keeps it untouched until
+        the batch's results are out), or ``resident``, a [B,H,W,3] u8 device tensor, device to device."""
+        if io.get("mixed"):
+            if resident is not None:
+                raise ValueError("resident= batches have one size: a batch of different sizes has no one-size device tensor")
+            self._stage_ragged(io, images)
+        elif resident is not None:
+            io["src"].copy_(resident, non_blocking=True)
+        elif torch.is_tensor(images) and images.is_pinned():
+            io["src"].copy_(images, non_blocking=True)
+        else:
+            for i, im in enumerate(images):
+                io["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
+            io["src"].copy_(io["host"], non_blocking=True)
+
+    @staticmethod
+    def _stage_ragged(io, images):
+        """Pack the screenshots and the batch's small data into the slot's pinned buffers and copy both to the device (two
+        H2D copies)."""
+        mb = io["batch"]
+        assert len(images) == io["B"] == len(mb["geom"])
         hv, host = io["host_views"], io["host"]
         hv["desc"].numpy()[:] = mb["desc"]
         g = np.asarray(mb["geom"], dtype=np.float64)
@@ -266,34 +296,28 @@ class B200YOLOv9Detector:
         io["small"][:n_small].copy_(io["host_small"][:n_small], non_blocking=True)
         n_src = mb["need"][0]
         io["src"][:n_src].copy_(host[:n_src], non_blocking=True)
-        io["sizes"] = [tuple(x[:2]) for x in mb["geom"]]
 
-    def detect_device_mixed(self, io, sizes, conf, iou, max_det):
-        """After :meth:`stage_mixed`, on the same stream: ragged letterbox -> forward -> decode -> NMS (no host sync)."""
-        assert [tuple(s) for s in sizes] == io["sizes"]
+    def detect(self, io, conf, iou, max_det):
+        """After :meth:`stage`, on the same stream: letterbox (the ragged kernel for a batch of different sizes) -> YOLOv9-E
+        forward -> decode -> NMS, outputs in the slot (no host sync)."""
         plan: YoloPlan = io["plan"]
-        tw, th = io["canvas"]
-        ops.letterbox_batch(io["src"], len(sizes), io["host_views"]["desc"], io["desc"], io["tables"], tw, th, io["tmp"],
-                            plan.canvas)
-        self._forward_nms(io, len(sizes), conf, iou, max_det)
-
-    def detect_device(self, io, B, H, W, conf, iou, max_det):
-        """Device-resident u8 images in io['src'] -> NMS outputs in io (no host sync)."""
-        plan: YoloPlan = io["plan"]
-        tw, th, scale, rw, rh, pl, pt = io["geom"]
-        ops.letterbox(io["src"], B, H, W, rw, rh, tw, th, pl, pt, io["tmp"], plan.canvas)
-        self._forward_nms(io, B, conf, iou, max_det)
-
-    def _forward_nms(self, io, B, conf, iou, max_det):
-        plan: YoloPlan = io["plan"]
+        B = io["B"]
+        if io.get("mixed"):
+            tw, th = io["canvas"]
+            ops.letterbox_batch(io["src"], B, io["host_views"]["desc"], io["desc"], io["tables"], tw, th, io["tmp"],
+                                plan.canvas)
+        else:
+            H, W = io["src"].shape[1:3]
+            tw, th, scale, rw, rh, pl, pt = io["geom"]
+            ops.letterbox(io["src"], B, H, W, rw, rh, tw, th, pl, pt, io["tmp"], plan.canvas)
         plan.run()
         ops.yolo_decode(plan.cls_out, plan.box_out, plan.hw, self.weights.nc, B, float(conf), io["pad_l"], io["pad_t"],
                         io["scale"], io["cap"], io["cand_box"], io["cand_score"], io["cand_cls"], io["cand_count"])
         ops.batched_nms(io["cand_box"], io["cand_score"], io["cand_cls"], io["cand_count"], B, io["cap"], iou, max_det,
                         io["img_w"], io["img_h"], io["keep"], io["out_box"], io["out_score"], io["out_count"])
 
-    def filter_device(self, io, B, H, W, ocr_elems, iou_threshold, max_det=300) -> bool:
-        """After :meth:`detect_device`, on the same stream: the reference's overlap filter (ref:util/utils.py:241-319,
+    def filter_device(self, io, ocr_elems, iou_threshold, max_det=300) -> bool:
+        """After :meth:`detect`, on the same stream: the reference's overlap filter (ref:util/utils.py:241-319,
         :411-415, :444-451) on the device -> per-icon state, OCR label masks / removed flags and the batch's crop list, plus
         the async D2H of the flags into this io slot's pinned mirrors.  ``ocr_elems[i]`` = host_glue.ocr_elements(...) of
         screenshot i (the strings stay on the host).  Returns False -- nothing launched -- when a screenshot has more OCR boxes
@@ -308,9 +332,9 @@ class B200YOLOv9Detector:
                 hr[i, :len(e)] = torch.tensor([x["bbox"] for x in e], dtype=torch.float32)
         io["ocr_ratio"].copy_(hr, non_blocking=True)
         io["ocr_count"].copy_(hc, non_blocking=True)
-        ops.overlap_filter(io["out_box"], io["out_count"], B, max_det, io["img_w"], io["img_h"], io["ocr_ratio"], io["ocr_count"],
-                           mo, float(iou_threshold), io["icon_state"], io["label_mask"], io["ocr_removed"], io["icon_ratio"],
-                           io["crop_box"], io["crop_img"], io["crop_counts"], io["arrive"])
+        ops.overlap_filter(io["out_box"], io["out_count"], len(ocr_elems), max_det, io["img_w"], io["img_h"], io["ocr_ratio"],
+                           io["ocr_count"], mo, float(iou_threshold), io["icon_state"], io["label_mask"], io["ocr_removed"],
+                           io["icon_ratio"], io["crop_box"], io["crop_img"], io["crop_counts"], io["arrive"])
         for h_, d_ in (("host_state", "icon_state"), ("host_mask", "label_mask"), ("host_removed", "ocr_removed"),
                        ("host_ratio", "icon_ratio"), ("host_crop_counts", "crop_counts")):
             io[h_].copy_(io[d_], non_blocking=True)
@@ -336,24 +360,13 @@ class B200YOLOv9Detector:
     @torch.inference_mode()
     def predict_batch(self, images: Sequence[np.ndarray], conf=0.25, imgsz=640, iou=0.7, max_det=300) -> List[Result]:
         """u8 HWC images -> one Result per image (one H2D copy of the screenshots, one D2H of the counts).  Screenshots of
-        different sizes share one batch through the ragged letterbox; same-size ones take the one-size path."""
-        B = len(images)
-        if self.is_mixed(list(images)):
-            with self._lock, torch.cuda.device(self.device):
-                mb = self.plan_mixed([im.shape[:2] for im in images], imgsz)
-                io = self._get_io_mixed(B, imgsz, max_det)
-                self.reserve_mixed(io, mb)
-                self.stage_mixed(io, mb, images)
-                self.detect_device_mixed(io, [im.shape[:2] for im in images], conf, iou, max_det)
-                return self._results(io)
-        H, W = images[0].shape[:2]
+        different sizes share one batch through the ragged letterbox."""
+        for im in images:
+            assert im.ndim == 3 and im.shape[2] == 3 and im.dtype == np.uint8
         with self._lock, torch.cuda.device(self.device):
-            io = self._get_io(B, H, W, imgsz, max_det)
-            for i, im in enumerate(images):
-                assert im.shape == (H, W, 3) and im.dtype == np.uint8
-                io["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
-            io["src"].copy_(io["host"], non_blocking=True)
-            self.detect_device(io, B, H, W, conf, iou, max_det)
+            io = self.io_slot([im.shape[:2] for im in images], imgsz, max_det)
+            self.stage(io, images)
+            self.detect(io, conf, iou, max_det)
             return self._results(io)
 
     def _results(self, io):

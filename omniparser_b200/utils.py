@@ -82,25 +82,100 @@ _HOST_GLUE = bool(os.environ.get("B2P_HOST_GLUE"))
 def _check_crop_status(status: torch.Tensor) -> None:
     """b2p_crop_resize flags crops whose truncated box is empty.  The reference silently skips such a crop
     (ref:util/utils.py:104-105) and then mis-assigns every later caption; int_box_area > 0 (:444-445) makes it impossible
-    on this path, so a flagged crop is a bug and raises (read after the ids' D2H sync: no extra synchronisation)."""
+    on this path, so a flagged crop is a bug and raises.  ``status`` is the host copy, made on the stream before the
+    ids' D2H sync: checking it costs no kernel and no extra synchronisation."""
     bad = int(status.count_nonzero().item())
     if bad:
         raise RuntimeError(f"{bad} crop boxes were empty after truncation (status flags of b2p_crop_resize)")
 
 
-def _crop_meta(model: B200YOLOv9Detector, io_, B, H, W, *key):
-    """(img_hw, img_off) of b2p_crop_resize for a batch's screenshots in io_["src"]: a ragged batch's are filled per batch in
-    its io slot; a one-size batch's are built once per (B, H, W, *key) and cached on the detector handle."""
-    if io_.get("mixed"):
-        return io_["meta_hw"], io_["meta_off"]
-    key = ("crop_meta", B, H, W) + key
-    meta = model._io.get(key)
-    if meta is None:
-        dev = model.device
-        meta = dict(hw=torch.tensor([[H, W]] * B, dtype=torch.int32, device=dev),
-                    off=torch.tensor([i * H * W * 3 for i in range(B)], dtype=torch.int64, device=dev))
-        model._io[key] = meta
-    return meta["hw"], meta["off"]
+def _detect(model: B200YOLOv9Detector, io_, sizes, ocr, conf, iou_threshold):
+    """Stage 1, on the current stream, after ``model.stage``: detection, the overlap filter on the device (unless
+    B2P_HOST_GLUE is set or a screenshot has more OCR boxes than the kernel takes), then async copies of the counts, boxes
+    and candidate counts into the slot's pinned mirrors and an event behind them (no host sync) -> the batch's handle."""
+    model.detect(io_, conf, 0.1, 300)
+    ocr_elems, on_device = None, False
+    if not _HOST_GLUE:
+        ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / torch.Tensor([w, h, w, h])).tolist() if ob else None, tx, w, h)
+                     for (h, w), (tx, ob) in zip(sizes, ocr)]   # :437-444
+        on_device = model.filter_device(io_, ocr_elems, iou_threshold, 300)
+    io_["host_count"].copy_(io_["out_count"], non_blocking=True)
+    if not on_device:
+        io_["host_box"].copy_(io_["out_box"], non_blocking=True)
+    io_["host_cand"].copy_(io_["cand_count"], non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record()
+    return dict(io=io_, ev=ev, sizes=sizes, ocr_elems=ocr_elems, on_device=on_device)
+
+
+def _host_lists(model: B200YOLOv9Detector, h, ocr, iou_threshold, det_override=None):
+    """Stage 2, after stage 1's event: the box counts and the crop list of a batch.  When the overlap filter ran on the
+    device, the crop list stays there and the element lists are built later from its flags (:func:`_elements`); otherwise
+    the reference's host list logic runs per screenshot.  ``det_override`` (tests) replaces the detector's boxes."""
+    io_ = h["io"]
+    if det_override is None:
+        counts, boxes = io_["host_count"].tolist(), io_["host_box"]
+        model.check_capacity(io_["host_cand"], io_["cap"])
+    else:
+        counts = [len(b) for b in det_override]
+        boxes = [torch.as_tensor(b, dtype=torch.float32).reshape(-1, 4) for b in det_override]
+    g = dict(h=h, counts=counts, all_elems=None, crop_boxes=[], crop_img=[])
+    if h["on_device"]:
+        g["n_crops"] = int(io_["host_crop_counts"][len(counts)])
+        return g
+    g["all_elems"] = []
+    for i, (hi, wi) in enumerate(h["sizes"]):
+        whwh = torch.Tensor([wi, hi, wi, hi])
+        xyxy = (boxes[i][:counts[i]] / whwh).tolist()                         # ref:util/utils.py:432
+        texts, obox = ocr[i]
+        oratio = (torch.tensor(obox) / whwh).tolist() if obox else None       # :437-442
+        elems, _ = host_glue.build_elements(xyxy, oratio, texts, wi, hi, iou_threshold)
+        g["all_elems"].append(elems)
+        for e in elems:
+            if e["content"] is None:
+                g["crop_boxes"].append(e["bbox"])
+                g["crop_img"].append(i)
+    g["n_crops"] = len(g["crop_boxes"])
+    return g
+
+
+def _elements(model: B200YOLOv9Detector, g):
+    """A batch's element lists; built here from the device overlap filter's flags if stage 2 left them to later."""
+    if g["all_elems"] is None:
+        h = g["h"]
+        g["all_elems"] = [model.elements_from_io(h["io"], i, n, h["ocr_elems"][i]) for i, n in enumerate(g["counts"])]
+    return g["all_elems"]
+
+
+def _cut_crops(gs, dst):
+    """Stage 3, on the current stream: the 64x64 crops of each batch of ``gs``, cut from its slot's screenshots into
+    consecutive row blocks of ``dst`` -> the status flags of b2p_crop_resize (see :func:`_check_crop_status`)."""
+    status = torch.zeros((sum(g["n_crops"] for g in gs),), dtype=torch.int32, device=dst.device)
+    off = 0
+    for g in gs:
+        n, io_ = g["n_crops"], g["h"]["io"]
+        if not n:
+            continue
+        if g["h"]["on_device"]:
+            boxes, img = io_["crop_box"], io_["crop_img"]
+        else:
+            boxes = torch.tensor(g["crop_boxes"], dtype=torch.float32).to(dst.device, non_blocking=True)
+            img = torch.tensor(g["crop_img"], dtype=torch.int32).to(dst.device, non_blocking=True)
+        ops.crop_resize(io_["src"], io_["meta_hw"], io_["meta_off"], boxes, img, n, 64, dst[off:], status[off:])
+        off += n
+    return status
+
+
+def _results(processor, all_elems, ids):
+    """Stage 4: captions into the element lists -> per screenshot ``(elements, caption ids)``, ids in crop order."""
+    texts = [t.strip() for t in processor.batch_decode(ids, skip_special_tokens=True)] if ids is not None else []
+    out, k = [], 0
+    for elems in all_elems:
+        m = sum(1 for e in elems if e["content"] is None)
+        host_glue.fill_captions(elems, texts[k:k + m])
+        out.append((elems, ids[k:k + m] if ids is not None else torch.zeros((0, 1), dtype=torch.long)))
+        k += m
+    return out
 
 
 @torch.inference_mode()
@@ -119,97 +194,46 @@ def parse_screenshots(images: Sequence[np.ndarray], model: B200YOLOv9Detector, c
     caption model's ``beam_defaults``)."""
     bs = beam_settings(num_beams, False, early_stopping, length_penalty, 1, caption_model_processor["model"].beam_defaults)
     bs.pop("num_return_sequences")
-    B = len(images)
-    mixed = B200YOLOv9Detector.is_mixed(images)
-    if mixed and _skip_h2d:
+    sizes = [tuple(im.shape[:2]) for im in images]
+    if _skip_h2d and len(set(sizes)) > 1:
         raise ValueError("_skip_h2d takes screenshots of one size: a batch of different sizes has no resident one-size buffer")
-    H, W = (None, None) if mixed else images[0].shape[:2]
-    sizes = [tuple(im.shape[:2]) for im in images] if mixed else [(H, W)] * B
     cap_model: B200Florence2Model = caption_model_processor["model"]
-    processor = caption_model_processor["processor"]
     t0 = time.perf_counter()
     with model._lock, torch.cuda.device(model.device):   # io slot 0 / caption plan instance 0 are this handle's: one call at a time
-        if mixed:
-            mb = model.plan_mixed(sizes, imgsz)
-            io_ = model._get_io_mixed(B, imgsz, 300)
-            model.reserve_mixed(io_, mb)
-            model.stage_mixed(io_, mb, images)
-        else:
-            io_ = model._get_io(B, H, W, imgsz, 300)
-        if not mixed and not _skip_h2d:   # bench "value" leg: the u8 screenshots are already resident in io_["src"]
-            for i, im in enumerate(images):
-                io_["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
-            io_["src"].copy_(io_["host"], non_blocking=True)
-        whwh = [torch.Tensor([w, h, w, h]) for h, w in sizes]
-        ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / whwh[i]).tolist() if ob else None, tx, sizes[i][1], sizes[i][0])
-                     for i, (tx, ob) in enumerate(ocr)]   # :437-444
-        on_device = False
+        io_ = model.io_slot(sizes, imgsz, 300)
+        if not _skip_h2d:   # bench "value" leg: the u8 screenshots are already resident in io_["src"]
+            model.stage(io_, images)
         if _det_override is None:
-            if mixed:
-                model.detect_device_mixed(io_, sizes, BOX_TRESHOLD, 0.1, 300)
-            else:
-                model.detect_device(io_, B, H, W, BOX_TRESHOLD, 0.1, 300)
-            on_device = not _HOST_GLUE and model.filter_device(io_, B, H, W, ocr_elems, iou_threshold, 300)
-            counts = io_["out_count"].cpu().tolist()                   # D2H #1 (sync; the filter's flags ride along)
-            boxes = None if on_device else io_["out_box"].cpu()
-            model.check_capacity(io_["cand_count"].cpu(), io_["cap"])
+            h = _detect(model, io_, sizes, ocr, BOX_TRESHOLD, iou_threshold)
+            h["ev"].synchronize()
         else:   # tests: inject detector output (e.g. the golden boxes) to pin the stages after it exactly
-            counts = [len(b) for b in _det_override]
-            boxes = [torch.as_tensor(b, dtype=torch.float32).reshape(-1, 4) for b in _det_override]
+            h = dict(io=io_, sizes=sizes, on_device=False)
         t1 = time.perf_counter()
-        all_elems, crop_boxes, crop_img = [], [], []
-        if on_device:
-            # overlap filter ran on the GPU (b2p_overlap_filter): element lists from its flags, crop list already on the device
-            for i in range(B):
-                all_elems.append(model.elements_from_io(io_, i, counts[i], ocr_elems[i]))
-            n = int(io_["host_crop_counts"][B])
-        else:
-            for i in range(B):
-                xyxy = (boxes[i][:counts[i]] / whwh[i]).tolist()           # ref:util/utils.py:432
-                texts, obox = ocr[i]
-                oratio = (torch.tensor(obox) / whwh[i]).tolist() if obox else None   # :437-442
-                elems, start = host_glue.build_elements(xyxy, oratio, texts, sizes[i][1], sizes[i][0], iou_threshold)
-                all_elems.append(elems)
-                for e in elems:
-                    if e["content"] is None:
-                        crop_boxes.append(e["bbox"])
-                        crop_img.append(i)
-            n = len(crop_boxes)
+        g = _host_lists(model, h, ocr, iou_threshold, _det_override)
+        n = g["n_crops"]
         t2 = time.perf_counter()
         ids = None
         if n:
           with cap_model._lock:   # plan instance 0 of the caption handle (also what model.generate() uses)
-            dev = model.device
             if caption_size == 64:
                 plan = cap_model.plan_for(n, max_new_tokens, prompt_ids, **bs)
-                crops_dst = plan.crops
+                crops = plan.crops
             else:
-                crops_dst = torch.empty((n, 64, 64, 3), dtype=torch.uint8, device=dev)
-            if on_device:
-                d_boxes, d_bimg = io_["crop_box"], io_["crop_img"]
-            else:
-                d_boxes = torch.tensor(crop_boxes, dtype=torch.float32).to(dev, non_blocking=True)
-                d_bimg = torch.tensor(crop_img, dtype=torch.int32).to(dev, non_blocking=True)
-            hw, off = _crop_meta(model, io_, B, H, W)
-            status = torch.zeros((n,), dtype=torch.int32, device=dev)
-            ops.crop_resize(io_["src"], hw, off, d_boxes, d_bimg, n, 64, crops_dst, status)
+                crops = torch.empty((n, 64, 64, 3), dtype=torch.uint8, device=model.device)
+            status = _cut_crops([g], crops)
             if caption_size == 64:
-                ids = cap_model.generate_from_device_crops(plan, n).cpu()  # D2H #2 (sync)
+                ids = cap_model.generate_from_device_crops(plan, n)
             else:
-                ids = cap_model.generate_chunked(crops_dst, max_new_tokens, prompt_ids, from_resized=False, **bs).cpu()
+                ids = cap_model.generate_chunked(crops, max_new_tokens, prompt_ids, from_resized=False, **bs)
+            _elements(model, g)   # device overlap filter: element lists from its flags, while the GPU captions
+            status = status.to("cpu", non_blocking=True)   # completed by the ids' D2H sync below
+            ids = ids.cpu()
             _check_crop_status(status)
+        all_elems = _elements(model, g)
         t3 = time.perf_counter()
-    out = []
-    k = 0
-    texts_all = processor.batch_decode(ids, skip_special_tokens=True) if ids is not None else []
-    texts_all = [t.strip() for t in texts_all]
-    for i in range(B):
-        m = sum(1 for e in all_elems[i] if e["content"] is None)
-        host_glue.fill_captions(all_elems[i], texts_all[k:k + m])
-        out.append((all_elems[i], ids[k:k + m] if ids is not None else torch.zeros((0, 1), dtype=torch.long)))
-        k += m
+    out = _results(caption_model_processor["processor"], all_elems, ids)
     if timings is not None:
-        timings.update(detect_s=t1 - t0, glue_s=t2 - t1, caption_s=t3 - t2, n_boxes=sum(counts), n_crops=n)
+        timings.update(detect_s=t1 - t0, glue_s=t2 - t1, caption_s=t3 - t2, n_boxes=sum(g["counts"]), n_crops=n)
     return out
 
 
@@ -260,171 +284,54 @@ class PipelinedParser:
         self.group = max(1, int(caption_group))
 
     @torch.inference_mode()
-    def _submit(self, slot: int, images, resident_src=None, ocr=None, mb=None):
+    def _submit(self, io_, images, resident_src, ocr):
+        """Stage 1 (submit thread, detection stream): the batch into its io slot, detection, the device overlap filter."""
         torch.cuda.set_device(self.model.device)   # runs on the worker thread: device and inference mode are thread-local
-        B = len(images)
-        m = self.model
-        if mb is not None:   # screenshots of different sizes (run() has sized the slot: see _ensure_io)
-            if resident_src is not None:
-                raise ValueError("resident= batches have one size: a batch of different sizes has no one-size device tensor")
-            sizes = [tuple(im.shape[:2]) for im in images]
-            H = W = None
-            io_ = m._get_io_mixed(B, self.imgsz, 300, slot)
-            assert not m.mixed_grow_needed(io_, mb)
-            m.reserve_mixed(io_, mb)
-        else:
-            H, W = images[0].shape[:2]
-            sizes = [(H, W)] * B
-            io_ = m._get_io(B, H, W, self.imgsz, 300, slot)
         with torch.cuda.stream(self.s_det):
-            if mb is not None:
-                m.stage_mixed(io_, mb, images)
-                m.detect_device_mixed(io_, sizes, self.conf, 0.1, 300)
-            else:
-                if resident_src is not None:
-                    io_["src"].copy_(resident_src, non_blocking=True)
-                elif torch.is_tensor(images) and images.is_pinned():
-                    # caller-owned page-locked [B,H,W,3] u8 batch: DMA straight from it (it must stay untouched until the
-                    # batch's result has been yielded); pageable numpy screenshots go through the slot's pinned staging copy
-                    io_["src"].copy_(images, non_blocking=True)
-                else:
-                    for i, im in enumerate(images):
-                        io_["host"][i].copy_(torch.from_numpy(np.ascontiguousarray(im)))
-                    io_["src"].copy_(io_["host"], non_blocking=True)
-                m.detect_device(io_, B, H, W, self.conf, 0.1, 300)
-            ocr_elems, on_device = None, False
-            if ocr is not None and not _HOST_GLUE:
-                # overlap filter on the device, right behind NMS on the detector's stream (no host round trip in between)
-                whwh = [torch.Tensor([w, h, w, h]) for h, w in sizes]
-                ocr_elems = [host_glue.ocr_elements((torch.tensor(ob) / whwh[i]).tolist() if ob else None, tx, sizes[i][1], sizes[i][0])
-                             for i, (tx, ob) in enumerate(ocr)]
-                on_device = m.filter_device(io_, B, H, W, ocr_elems, self.iou_thr, 300)
-            io_["host_count"].copy_(io_["out_count"], non_blocking=True)
-            if not on_device:
-                io_["host_box"].copy_(io_["out_box"], non_blocking=True)
-            io_["host_cand"].copy_(io_["cand_count"], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(self.s_det)
-        return dict(io=io_, ev=ev, B=B, H=H, W=W, sizes=sizes, ocr_elems=ocr_elems, on_device=on_device)
+            self.model.stage(io_, images, resident_src)
+            return _detect(self.model, io_, [tuple(im.shape[:2]) for im in images], ocr, self.conf, self.iou_thr)
 
     def _glue(self, h, ocr):
         """Stage 2 (caller's thread): wait for the detector's boxes, run the reference's host list logic."""
-        io_, B, H, W = h["io"], h["B"], h["H"], h["W"]
         t0 = time.perf_counter()
         h["ev"].synchronize()
         t1 = time.perf_counter()
-        counts = io_["host_count"].tolist()
-        self.model.check_capacity(io_["host_cand"], io_["cap"])
-        all_elems, crop_boxes, crop_img = [], [], []
-        if h.get("on_device"):
-            # the device filter's flags arrived with the counts: element lists are built later, on the caption thread (they are
-            # only needed for the result); the crop list stays on the device
-            n_crops = int(io_["host_crop_counts"][B])
-            all_elems = None
-        else:
-            boxes = io_["host_box"]
-            for i, (hi, wi) in enumerate(h["sizes"]):
-                whwh = torch.Tensor([wi, hi, wi, hi])
-                xyxy = (boxes[i][:counts[i]] / whwh).tolist()
-                texts, obox = ocr[i]
-                oratio = (torch.tensor(obox) / whwh).tolist() if obox else None
-                elems, _ = host_glue.build_elements(xyxy, oratio, texts, wi, hi, self.iou_thr)
-                all_elems.append(elems)
-                for e in elems:
-                    if e["content"] is None:
-                        crop_boxes.append(e["bbox"])
-                        crop_img.append(i)
-            n_crops = len(crop_boxes)
+        g = _host_lists(self.model, h, ocr, self.iou_thr)
         t2 = time.perf_counter()
         tm = self.timings
         tm["detect_wait_s"] += t1 - t0; tm["glue_s"] += t2 - t1
-        tm["n_boxes"] += sum(counts); tm["n_crops"] += n_crops; tm["batches"] += 1
-        lane = (self._job // self.group) % self.lanes   # the batches of one caption group share a lane
+        tm["n_boxes"] += sum(g["counts"]); tm["n_crops"] += g["n_crops"]; tm["batches"] += 1
+        g["lane"] = (self._job // self.group) % self.lanes   # the batches of one caption group share a lane
         self._job += 1
-        return dict(h=h, all_elems=all_elems, crop_boxes=crop_boxes, crop_img=crop_img, lane=lane, n_crops=n_crops, counts=counts)
-
-    @torch.inference_mode()
-    def _caption(self, g):
-        """Stage 3 (caption thread, stream B): crop+resize from the resident screenshots, Florence-2 greedy decode,
-        token ids back to the host, captions into the element lists."""
-        torch.cuda.set_device(self.model.device)
-        h, all_elems, crop_boxes, crop_img = g["h"], g["all_elems"], g["crop_boxes"], g["crop_img"]
-        io_, B, H, W = h["io"], h["B"], h["H"], h["W"]
-        model, cap_model, processor = self.model, self.cmp["model"], self.cmp["processor"]
-        n = g["n_crops"]
-        t2 = time.perf_counter()
-        ids = None
-        if n:
-            dev = model.device
-            lane = g.get("lane", 0)
-            with torch.cuda.stream(self.s_caps[lane]):
-                plan = cap_model.plan_for(n, self.T, self.prompt, instance=lane)
-                if h.get("on_device"):
-                    d_boxes, d_bimg = io_["crop_box"], io_["crop_img"]
-                else:
-                    d_boxes = torch.tensor(crop_boxes, dtype=torch.float32).to(dev, non_blocking=True)
-                    d_bimg = torch.tensor(crop_img, dtype=torch.int32).to(dev, non_blocking=True)
-                hw, off = _crop_meta(model, io_, B, H, W, lane)
-                status = torch.zeros((n,), dtype=torch.int32, device=dev)
-                ops.crop_resize(io_["src"], hw, off, d_boxes, d_bimg, n, 64, plan.crops, status)
-                ids = cap_model.generate_from_device_crops(plan, n)
-                if all_elems is None:   # device overlap filter: element lists from its flags, while the GPU captions
-                    all_elems = [model.elements_from_io(io_, i, g["counts"][i], h["ocr_elems"][i]) for i in range(B)]
-                ids = ids.cpu()
-                _check_crop_status(status)
-        if all_elems is None:
-            all_elems = [model.elements_from_io(io_, i, g["counts"][i], h["ocr_elems"][i]) for i in range(B)]
-        t3 = time.perf_counter()
-        texts_all = [t.strip() for t in processor.batch_decode(ids, skip_special_tokens=True)] if ids is not None else []
-        out, k = [], 0
-        for i in range(B):
-            mcap = sum(1 for e in all_elems[i] if e["content"] is None)
-            host_glue.fill_captions(all_elems[i], texts_all[k:k + mcap])
-            out.append((all_elems[i], ids[k:k + mcap] if ids is not None else torch.zeros((0, 1), dtype=torch.long)))
-            k += mcap
-        with self._tm_lock:
-            self.timings["caption_s"] += t3 - t2
-        return out
+        return g
 
     @torch.inference_mode()
     def _caption_group(self, gs):
-        """caption_group > 1: one Florence-2 pass over the crops of several batches (same lane); returns the per-batch
-        results in order.  Row blocks of ``plan.crops`` are filled batch by batch from each batch's resident screenshots."""
+        """Stage 3 (caption thread, the lane's stream): one Florence-2 pass over the crops of up to ``caption_group``
+        batches, cut batch by batch into row blocks of ``plan.crops`` from each batch's resident screenshots; token ids back
+        to the host, captions into the element lists -> the per-batch results, in order."""
         torch.cuda.set_device(self.model.device)
-        model, cap_model, processor = self.model, self.cmp["model"], self.cmp["processor"]
+        model, cap_model = self.model, self.cmp["model"]
         lane = gs[0]["lane"]
-        counts = [g["n_crops"] for g in gs]
-        n = sum(counts)
-        for g in gs:
-            if g["all_elems"] is None:
-                hh = g["h"]
-                g["all_elems"] = [model.elements_from_io(hh["io"], i, g["counts"][i], hh["ocr_elems"][i]) for i in range(hh["B"])]
+        n = sum(g["n_crops"] for g in gs)
         t2 = time.perf_counter()
         ids = None
         if n:
-            dev = model.device
             with torch.cuda.stream(self.s_caps[lane]):
                 plan = cap_model.plan_for(n, self.T, self.prompt, instance=lane)
-                off = 0
-                for g, ng in zip(gs, counts):
-                    if not ng:
-                        continue
-                    io_, B, H, W = g["h"]["io"], g["h"]["B"], g["h"]["H"], g["h"]["W"]
-                    if g["h"].get("on_device"):
-                        d_boxes, d_bimg = io_["crop_box"], io_["crop_img"]
-                    else:
-                        d_boxes = torch.tensor(g["crop_boxes"], dtype=torch.float32).to(dev, non_blocking=True)
-                        d_bimg = torch.tensor(g["crop_img"], dtype=torch.int32).to(dev, non_blocking=True)
-                    hw, moff = _crop_meta(model, io_, B, H, W, lane)
-                    status = torch.zeros((ng,), dtype=torch.int32, device=dev)
-                    ops.crop_resize(io_["src"], hw, moff, d_boxes, d_bimg, ng, 64, plan.crops[off:], status)
-                    off += ng
-                ids = cap_model.generate_from_device_crops(plan, n).cpu()
+                status = _cut_crops(gs, plan.crops)
+                ids = cap_model.generate_from_device_crops(plan, n)
+                for g in gs:   # device overlap filter: element lists from its flags, while the GPU captions
+                    _elements(model, g)
+                status = status.to("cpu", non_blocking=True)   # completed by the ids' D2H sync below
+                ids = ids.cpu()
+                _check_crop_status(status)
+        for g in gs:
+            _elements(model, g)
         t3 = time.perf_counter()
         outs, off = [], 0
-        for g, ng in zip(gs, counts):
-            all_elems, B = g["all_elems"], g["h"]["B"]
-            ids_b = None
+        for g in gs:
+            ng, ids_b = g["n_crops"], None
             if ng:
                 ids_b = ids[off:off + ng]
                 # HF would have stopped this batch alone at the first step where all ITS rows had finished
@@ -432,20 +339,10 @@ class PipelinedParser:
                 if done_at is not None:
                     ids_b = ids_b[:, :done_at + 1]
                 off += ng
-            texts_all = [t.strip() for t in processor.batch_decode(ids_b, skip_special_tokens=True)] if ids_b is not None else []
-            out, k = [], 0
-            for i in range(B):
-                mcap = sum(1 for e in all_elems[i] if e["content"] is None)
-                host_glue.fill_captions(all_elems[i], texts_all[k:k + mcap])
-                out.append((all_elems[i], ids_b[k:k + mcap] if ids_b is not None else torch.zeros((0, 1), dtype=torch.long)))
-                k += mcap
-            outs.append(out)
+            outs.append(_results(self.cmp["processor"], g["all_elems"], ids_b))
         with self._tm_lock:
             self.timings["caption_s"] += t3 - t2
         return outs
-
-    def _finish(self, h, ocr):
-        return self._caption(self._glue(h, ocr))
 
     @torch.inference_mode()
     def run(self, batches, resident=None):
@@ -462,10 +359,9 @@ class PipelinedParser:
             cur = next(it, None)
             if cur is None:
                 return
-            slot = 0
-            mb = self._ensure_io(slot, cur[0], ())
-            h = self._submit(slot, cur[0], next(rit) if rit is not None else None, cur[1], **({} if mb is None else dict(mb=mb)))
             pending = deque()
+            slot = 0
+            h = self._submit(self._ensure_io(slot, cur[0], pending), cur[0], next(rit) if rit is not None else None, cur[1])
             grp = []
             while cur is not None:
                 nxt = next(it, None)
@@ -474,20 +370,14 @@ class PipelinedParser:
                     # slots alive at once: lanes*group in caption + up to group-1 glued batches waiting for their group
                     # + the batch in the host list logic + the batch in detection  (= lanes + 2 when group == 1)
                     slot = (slot + 1) % (self.lanes * self.group + self.group + 1)
-                    mb = self._ensure_io(slot, nxt[0], pending)
-                    fut = self._pool.submit(self._submit, slot, nxt[0], next(rit) if rit is not None else None, nxt[1],
-                                            **({} if mb is None else dict(mb=mb)))
-                g = self._glue(h, cur[1])
-                if self.group == 1:
-                    self._ensure_plan(g, pending, fut)
-                    pending.append(self._cap_pools[g["lane"]].submit(self._caption, g))
-                else:
-                    grp.append(g)
-                    if len(grp) == self.group or nxt is None:
-                        self._ensure_plan(dict(n_crops=sum(x["n_crops"] for x in grp), lane=grp[0]["lane"]), pending, fut)
-                        fc = self._cap_pools[grp[0]["lane"]].submit(self._caption_group, grp)
-                        pending.extend(_Member(fc, j) for j in range(len(grp)))
-                        grp = []
+                    io_ = self._ensure_io(slot, nxt[0], pending)
+                    fut = self._pool.submit(self._submit, io_, nxt[0], next(rit) if rit is not None else None, nxt[1])
+                grp.append(self._glue(h, cur[1]))
+                if len(grp) == self.group or nxt is None:
+                    self._ensure_plan(dict(n_crops=sum(x["n_crops"] for x in grp), lane=grp[0]["lane"]), pending, fut)
+                    fc = self._cap_pools[grp[0]["lane"]].submit(self._caption_group, grp)
+                    pending.extend(_Member(fc, j) for j in range(len(grp)))
+                    grp = []
                 while len(pending) > self.lanes * self.group:
                     yield pending.popleft().result()
                 hn = fut.result() if fut is not None else None
@@ -518,20 +408,12 @@ class PipelinedParser:
             torch.cuda.synchronize()
 
     def _ensure_io(self, slot, images, pending):
-        """A batch of screenshots of different sizes -> its letterbox plan (None for a one-size batch).  When the batch does
-        not fit the buffers its io slot already holds, the pipeline is drained (every batch in flight finished, device
-        synchronised) before the slot grows: the freed buffers may still be read by another stream until then."""
-        if not B200YOLOv9Detector.is_mixed(images):
-            return None
-        m = self.model
-        mb = m.plan_mixed([tuple(im.shape[:2]) for im in images], self.imgsz)
-        io_ = m._get_io_mixed(len(images), self.imgsz, 300, slot)
-        if m.mixed_grow_needed(io_, mb):
+        """A batch's io slot (caller's thread).  When a batch of different sizes does not fit the buffers its slot already
+        holds, every batch in flight is finished before the slot grows (see B200YOLOv9Detector.io_slot)."""
+        def drain():
             for p in pending:
                 p.result()
-            torch.cuda.synchronize()
-            m.reserve_mixed(io_, mb)
-        return mb
+        return self.model.io_slot([tuple(im.shape[:2]) for im in images], self.imgsz, 300, slot, drain)
 
     def _ensure_plan(self, g, pending, fut):
         """First batch of a crop-count bucket on a lane: drain the pipeline and build + capture the caption plan with

@@ -5,7 +5,7 @@
   reported buffer sizes, and degenerate geometry / a short table buffer are refused before anything is written;
 * a dry run of `PipelinedParser` over mixed-size batches (the recording C library of test_plan_dryrun_cpu.py and a fake
   detector with the ragged-batch methods): order, the crop metadata each `b2p_crop_resize` call gets, io slot growth only
-  with the pipeline drained, and a bounded number of io slots;
+  with the pipeline drained, a bounded number of io slots, and the same results as `parse_screenshots`;
 * `BatchingOmniparser`: requests of three sizes share one batch."""
 import ctypes
 import threading
@@ -149,8 +149,6 @@ class _MixedFakeDetector:
     (B, slot) whose capacity (src bytes) grows.  'Detects' 3 boxes per screenshot; records what the pipeline asks of it."""
 
     def __init__(self, in_flight):
-        from omniparser_b200.detector import B200YOLOv9Detector
-        self.is_mixed = B200YOLOv9Detector.is_mixed
         self.device = torch.device("cpu")
         self._io = {}
         self._lock = threading.RLock()
@@ -161,64 +159,51 @@ class _MixedFakeDetector:
     def check_capacity(cand_count_host, cap):
         pass
 
-    def filter_device(self, io, B_, H_, W_, ocr_elems, iou_threshold, max_det=300):
+    def filter_device(self, io, ocr_elems, iou_threshold, max_det=300):
         return False
 
     def _buffers(self, B_, max_det=300):
         return dict(host_count=torch.zeros((B_,), dtype=torch.int32), host_box=torch.zeros((B_, max_det, 4)),
                     out_count=torch.zeros((B_,), dtype=torch.int32), out_box=torch.zeros((B_, max_det, 4)),
-                    cand_count=torch.zeros((B_,), dtype=torch.int32), host_cand=torch.zeros((B_,), dtype=torch.int32), cap=8400)
+                    cand_count=torch.zeros((B_,), dtype=torch.int32), host_cand=torch.zeros((B_,), dtype=torch.int32), cap=8400,
+                    B=B_)
 
-    def _get_io(self, B_, H_, W_, imgsz, max_det, slot=0):
-        key = (B_, H_, W_, slot)
-        if key not in self._io:
-            self._io[key] = dict(self._buffers(B_), src=torch.zeros((B_, H_, W_, 3), dtype=torch.uint8),
-                                 host=torch.zeros((B_, H_, W_, 3), dtype=torch.uint8))
-        return self._io[key]
-
-    @staticmethod
-    def plan_mixed(sizes, imgsz):
+    def io_slot(self, sizes, imgsz, max_det, slot=0, drain=None):
+        sizes = [tuple(s) for s in sizes]
+        B_ = len(sizes)
+        if len(set(sizes)) == 1:
+            H_, W_ = sizes[0]
+            key = (B_, H_, W_, slot)
+            if key not in self._io:
+                self._io[key] = dict(self._buffers(B_), src=torch.zeros((B_, H_, W_, 3), dtype=torch.uint8),
+                                     meta_hw=torch.tensor([[H_, W_]] * B_, dtype=torch.int32),
+                                     meta_off=torch.tensor([i * H_ * W_ * 3 for i in range(B_)], dtype=torch.int64))
+            return self._io[key]
         off = np.cumsum([0] + [3 * h * w for h, w in sizes])
-        return dict(sizes=list(sizes), off=off[:-1], need=(int(off[-1]), 0, 0))
-
-    def _get_io_mixed(self, B_, imgsz, max_det, slot=0):
-        key = ("mixed", B_, slot)
-        if key not in self._io:
-            self._io[key] = dict(self._buffers(B_), mixed=True, src=None, cap=8400, cap_src=0)
-        return self._io[key]
-
-    @staticmethod
-    def mixed_grow_needed(io, mb):
-        return io["src"] is not None and mb["need"][0] > io["cap_src"]
-
-    def reserve_mixed(self, io, mb):
-        if io["src"] is not None and mb["need"][0] <= io["cap_src"]:
-            return
-        if io["src"] is not None:
-            self.growths += 1
-            if self.in_flight():
-                self.bad_growths.append(self.in_flight())
-        io["cap_src"] = max(mb["need"][0], io["cap_src"] * 3 // 2)
-        io["src"] = torch.zeros((io["cap_src"],), dtype=torch.uint8)
-
-    def stage_mixed(self, io, mb, images):
-        assert mb["need"][0] <= io["cap_src"]
-        B_ = len(images)
-        io["meta_hw"] = torch.tensor(mb["sizes"], dtype=torch.int32)
-        io["meta_off"] = torch.tensor(mb["off"], dtype=torch.int64)
-        io["sizes"] = mb["sizes"]
-        assert B_ == len(mb["sizes"])
-
-    def detect_device_mixed(self, io, sizes, conf, iou, max_det):
-        assert [tuple(s) for s in sizes] == io["sizes"]
-        self._detect(io, sizes)
-
-    def detect_device(self, io, B_, H_, W_, conf, iou, max_det):
-        self._detect(io, [(H_, W_)] * B_)
+        io = self._io.setdefault(("mixed", B_, slot), dict(self._buffers(B_), mixed=True, src=None, cap_src=0))
+        if io["src"] is None or off[-1] > io["cap_src"]:
+            if io["src"] is not None:
+                if drain is not None:
+                    drain()
+                self.growths += 1
+                if self.in_flight():
+                    self.bad_growths.append(self.in_flight())
+            io["cap_src"] = max(int(off[-1]), io["cap_src"] * 3 // 2)
+            io["src"] = torch.zeros((io["cap_src"],), dtype=torch.uint8)
+        io["batch"] = dict(sizes=sizes, off=off[:-1])
+        return io
 
     @staticmethod
-    def _detect(io, sizes):
-        for i, (h, w) in enumerate(sizes):
+    def stage(io, images, resident=None):
+        if io.get("mixed"):
+            mb = io["batch"]
+            assert [tuple(im.shape[:2]) for im in images] == mb["sizes"]
+            io["meta_hw"] = torch.tensor(mb["sizes"], dtype=torch.int32)
+            io["meta_off"] = torch.tensor(mb["off"], dtype=torch.int64)
+
+    @staticmethod
+    def detect(io, conf, iou, max_det):
+        for i in range(io["B"]):
             for j in range(3):      # boxes inside every screenshot (the smallest is 200 x 120)
                 io["out_box"][i, j] = torch.tensor([10.0 + 50 * j, 10.0 + 5 * i, 50.0 + 50 * j, 60.0 + 5 * i])
             io["out_count"][i] = 3
@@ -243,7 +228,7 @@ def _mixed_batches(n, B_=3):
 
 
 @pytest.mark.parametrize("lanes,group", [(1, 1), (2, 1), (1, 2), (2, 2)])
-def test_pipelined_parser_mixed_dry_run(env, florence, lanes, group):
+def test_pipelined_parser_io_slot_dry_run(env, florence, lanes, group):
     from omniparser_b200.caption import B200Florence2Processor
     from omniparser_b200.utils import PipelinedParser
     busy = [0]
@@ -263,7 +248,7 @@ def test_pipelined_parser_mixed_dry_run(env, florence, lanes, group):
                 with lock:
                     busy[0] -= 1
         return w
-    pp._caption, pp._caption_group = tracked(pp._caption), tracked(pp._caption_group)
+    pp._caption_group = tracked(pp._caption_group)
     nb = 14
     batches = _mixed_batches(nb)
     got = list(pp.run(iter(batches)))
@@ -288,7 +273,7 @@ def test_pipelined_parser_mixed_dry_run(env, florence, lanes, group):
     assert len([k for k in det._io if k[0] == "mixed"]) <= n_slots
 
 
-def test_pipelined_parser_crop_meta_per_batch(env, florence):
+def test_pipelined_parser_slot_crop_meta_per_batch(env, florence):
     """each crop_resize call of a mixed batch reads that batch's (H, W) and offsets at call time"""
     from omniparser_b200 import utils as U
     from omniparser_b200.caption import B200Florence2Processor
@@ -310,12 +295,32 @@ def test_pipelined_parser_crop_meta_per_batch(env, florence):
     assert len(seen) == 6
     for (imgs, _), (hw, off) in zip(batches, seen):
         sizes = [list(im.shape[:2]) for im in imgs]
-        if det.is_mixed(imgs):
+        if len(set(map(tuple, sizes))) > 1:
             assert hw == sizes
             assert off == list(np.cumsum([0] + [3 * h * w for h, w in sizes])[:-1])
         else:
             h, w = sizes[0]
             assert hw == sizes and off == [i * 3 * h * w for i in range(len(imgs))]
+
+
+@pytest.mark.parametrize("group", [1, 2])
+def test_pipelined_parser_equals_parse_screenshots(env, florence, group):
+    """the two batch entry points share their stages: on the same one-size and mixed batches, PipelinedParser.run (two
+    lanes) returns what parse_screenshots returns batch by batch"""
+    from omniparser_b200.caption import B200Florence2Processor
+    from omniparser_b200.utils import PipelinedParser, parse_screenshots
+    det = _MixedFakeDetector(lambda: 0)
+    cmp_ = dict(model=_cap_model(florence), processor=B200Florence2Processor())
+    kw = dict(BOX_TRESHOLD=0.05, iou_threshold=0.7, max_new_tokens=3)
+    batches = _mixed_batches(6)
+    assert {len({im.shape for im in imgs}) > 1 for imgs, _ in batches} == {False, True}
+    ref = [parse_screenshots(imgs, det, cmp_, ocr, **kw) for imgs, ocr in batches]
+    got = list(PipelinedParser(det, cmp_, caption_lanes=2, caption_group=group, **kw).run(iter(batches)))
+    assert len(got) == len(ref)
+    for out, exp in zip(got, ref):
+        assert len(out) == len(exp)
+        for (elems, ids), (elems_ref, ids_ref) in zip(out, exp):
+            assert elems == elems_ref and torch.equal(ids, ids_ref) and ids.shape[0] == 3
 
 
 # ------------------------------------------------------------------------------------------------ server

@@ -1,7 +1,7 @@
 """CPU dry run of ``PipelinedParser`` end to end (threads, lanes, io slots, caption grouping): the CUDA library is the
 recorder of test_plan_dryrun_cpu.py (no arithmetic), the detector is a stub that "finds" fixed boxes, CUDA streams/events are
 dummies.  What is checked is the host-side plumbing the GPU tests cannot reach without hardware time: every code path of
-``_submit`` / ``_glue`` / ``_caption`` / ``_caption_group`` runs, results come back per batch in order with the right
+``_submit`` / ``_glue`` / ``_caption_group`` runs, results come back per batch in order with the right
 shapes, crops of a group land in consecutive row blocks of ONE plan, and the opt-in grouping launches fewer Florence passes."""
 import contextlib
 import ctypes as C
@@ -40,23 +40,31 @@ class _FakeDetector:
     def check_capacity(cand_count_host, cap):
         assert int(cand_count_host.max()) <= cap
 
-    def _get_io(self, B_, H_, W_, imgsz, max_det, slot=0):
+    def io_slot(self, sizes, imgsz, max_det, slot=0, drain=None):
+        (H_, W_), B_ = sizes[0], len(sizes)
         key = (B_, H_, W_, slot)
         if key not in self._io:
-            self._io[key] = dict(src=torch.zeros((B_, H_, W_, 3), dtype=torch.uint8), host=torch.zeros((B_, H_, W_, 3), dtype=torch.uint8),
+            self._io[key] = dict(src=torch.zeros((B_, H_, W_, 3), dtype=torch.uint8), B=B_,
                                  host_count=torch.zeros((B_,), dtype=torch.int32), host_box=torch.zeros((B_, max_det, 4)),
                                  out_count=torch.zeros((B_,), dtype=torch.int32), out_box=torch.zeros((B_, max_det, 4)),
-                                 cand_count=torch.zeros((B_,), dtype=torch.int32), host_cand=torch.zeros((B_,), dtype=torch.int32), cap=8400)
+                                 cand_count=torch.zeros((B_,), dtype=torch.int32), host_cand=torch.zeros((B_,), dtype=torch.int32), cap=8400,
+                                 meta_hw=torch.tensor([[H_, W_]] * B_, dtype=torch.int32),
+                                 meta_off=torch.tensor([i * H_ * W_ * 3 for i in range(B_)], dtype=torch.int64))
         return self._io[key]
 
-    def filter_device(self, io, B_, H_, W_, ocr_elems, iou_threshold, max_det=300):
+    @staticmethod
+    def stage(io, images, resident=None):
+        for i, im in enumerate(images):
+            io["src"][i].copy_(torch.from_numpy(im))
+
+    def filter_device(self, io, ocr_elems, iou_threshold, max_det=300):
         return False      # "more OCR boxes than the device filter takes": the pipeline runs the host list logic (host_glue)
 
-    def detect_device(self, io, B_, H_, W_, conf, iou, max_det):
+    def detect(self, io, conf, iou, max_det):
         with self.lock:
             k = 3 + self.n % 2
             self.n += 1
-        for i in range(B_):
+        for i in range(io["B"]):
             for j in range(k):
                 io["out_box"][i, j] = torch.tensor([20.0 + 60 * j, 30.0 + 10 * i, 60.0 + 60 * j, 80.0 + 10 * i])
             io["out_count"][i] = k
@@ -104,7 +112,7 @@ def _batches(n):
 
 
 @pytest.mark.parametrize("lanes,group", [(1, 1), (2, 1), (2, 2), (1, 3)])
-def test_pipelined_parser_host_plumbing(env, florence, lanes, group):
+def test_pipelined_parser_stage_plumbing(env, florence, lanes, group):
     from omniparser_b200.caption import B200Florence2Processor
     from omniparser_b200.utils import PipelinedParser
     det = _FakeDetector()
@@ -136,7 +144,7 @@ def test_pipelined_parser_host_plumbing(env, florence, lanes, group):
 
 
 @pytest.mark.parametrize("caption_size", [64, 768])
-def test_parse_screenshots_host_plumbing(env, florence, monkeypatch, caption_size):
+def test_parse_screenshots_stage_plumbing(env, florence, monkeypatch, caption_size):
     """the one-batch-at-a-time entry point, both caption modes (768: device resize + chunked generate)"""
     from omniparser_b200 import caption
     from omniparser_b200.caption import B200Florence2Processor

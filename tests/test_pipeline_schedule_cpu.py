@@ -34,6 +34,9 @@ class _Sched(PipelinedParser):
     def _ensure_plan(self, g, pending, fut):
         pass
 
+    def _ensure_io(self, slot, images, pending):
+        return slot
+
     def _submit(self, slot, images, resident_src=None, ocr=None):
         with self.lock:
             if slot in self.busy_slots:
@@ -63,24 +66,11 @@ class _Sched(PipelinedParser):
                 del self.busy_slots[g["h"]["slot"]]
         return batches
 
-    def _caption(self, g):
-        lane, batch = g["lane"], g["h"]["batch"]
-        with self.lock:
-            if lane in self.active_lanes:
-                self.errors.append(f"lane {lane}: batch {batch} started while batch {self.active_lanes[lane]} was in flight")
-            self.active_lanes[lane] = batch
-            self.max_parallel = max(self.max_parallel, len(self.active_lanes))
-        time.sleep(self.rng.choice([0.001, 0.004, 0.012]))   # uneven durations: the case that used to interleave
-        with self.lock:
-            del self.active_lanes[lane]
-            del self.busy_slots[g["h"]["slot"]]
-        return batch
-
 
 @pytest.mark.parametrize("group", [1, 2, 3])
 @pytest.mark.parametrize("lanes", [1, 2, 3])
 @pytest.mark.parametrize("seed", [0, 1])
-def test_schedule_invariants(lanes, seed, group):
+def test_schedule_invariants_through_caption_group(lanes, seed, group):
     s = _Sched(lanes, seed, group)
     n = 41
     out = list(s.run((i, None) for i in range(n)))

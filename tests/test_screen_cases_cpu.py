@@ -196,10 +196,10 @@ def test_geometry_accepts_one_pixel_results():
         assert _geometry(w, h, 640) == R.letterbox_geometry(w, h, 640)
 
 
-def test_more_ocr_boxes_than_the_device_filter_takes_go_to_the_host():
+def test_filter_device_leaves_more_ocr_boxes_than_it_takes_to_the_host():
     """the device filter takes up to 256 OCR boxes per screenshot (detector.OCR_CAP = host_glue.OCR_DEVICE_CAP);
     filter_device returns False, launching nothing, as soon as one screenshot of the batch has more"""
     from omniparser_b200.detector import B200YOLOv9Detector
     assert B200YOLOv9Detector.OCR_CAP == host_glue.OCR_DEVICE_CAP == S.MAX_OCR
     io = {"max_ocr": S.MAX_OCR}   # nothing else: any use of a device buffer would raise
-    assert B200YOLOv9Detector.filter_device(None, io, 2, S.H, S.W, [[{}] * 3, [{}] * (S.MAX_OCR + 1)], 0.7) is False
+    assert B200YOLOv9Detector.filter_device(None, io, [[{}] * 3, [{}] * (S.MAX_OCR + 1)], 0.7) is False

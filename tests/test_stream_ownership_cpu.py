@@ -249,13 +249,13 @@ class _YoloDetector(_FakeDetector):
         from omniparser_b200.yolo_engine import YoloPlan
         self.plan = YoloPlan(yolo_weights, 1, 64, 96, use_graph=True)
 
-    def detect_device(self, io, B_, H_, W_, conf, iou, max_det):
+    def detect(self, io, conf, iou, max_det):
         self.plan.run()
-        super().detect_device(io, B_, H_, W_, conf, iou, max_det)
+        super().detect(io, conf, iou, max_det)
 
 
 @pytest.mark.parametrize("lanes,group,parts", [(2, 2, 1), (3, 1, 1), (2, 1, 2)])
-def test_gemm_calls_carry_their_role_stream(env, florence, yolo_weights, monkeypatch, lanes, group, parts):
+def test_gemm_calls_of_each_stage_carry_their_role_stream(env, florence, yolo_weights, monkeypatch, lanes, group, parts):
     """Run the pipelined parser end to end with graphs on: every split-K-capable GEMM/conv call made inside a capture carries
     the capture stream of its engine and lane; every eager one carries the working stream of its stage, lane or decode
     chain -- never the default stream, never a capture stream."""
@@ -263,7 +263,7 @@ def test_gemm_calls_carry_their_role_stream(env, florence, yolo_weights, monkeyp
     rec, ts, pool = env
     if parts > 1:       # decode chains on their own streams: 128 crops per lane and batch
         monkeypatch.setenv("B2P_DECODE_PARTS", str(parts))
-        monkeypatch.setattr(_FakeDetector, "detect_device", _many_boxes)
+        monkeypatch.setattr(_FakeDetector, "detect", _many_boxes)
     monkeypatch.setattr(caption, "BUCKET", 32)
     cap = _cap_model(florence)
     cap.use_graph = True
@@ -308,9 +308,9 @@ def test_gemm_calls_carry_their_role_stream(env, florence, yolo_weights, monkeyp
     assert seen == {v[0] for v in capt.values()}, sorted(seen)
 
 
-def _many_boxes(self, io, B_, H_, W_, conf, iou, max_det):
+def _many_boxes(self, io, conf, iou, max_det):
     """65 boxes per screenshot (130 crops per batch of 2): enough rows for two decode chains"""
-    for i in range(B_):
+    for i in range(io["B"]):
         for j in range(65):
             x, y = 4 + 7 * (j % 13), 4 + 40 * (j // 13)
             io["out_box"][i, j] = torch.tensor([float(x), float(y) + i, float(x + 5), float(y + 30 + i)])
